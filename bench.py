@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — env-steps/s of the VMAS physics hot path behind ``Environment.step`` on B200.
+"""bench.py — env-steps/s of the VMAS physics hot path behind ``Environment.step`` on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (default): BASELINE.json configs[1] — scenario ``balance``, 32768 envs per GPU, 4 agents,
@@ -18,8 +18,14 @@ One JSON line is printed by rank 0:
 Timing: per-iteration CUDA events on the launching stream, summed; L2 is flushed (512 MiB
 memset) between iterations outside the brackets; max over ranks.
 
-``--impl reference`` times the oracle port of the path (the reference is pure Python and does not
-travel to the GPU box; the port issues the same eager torch op chain and is bit-identical to it,
+``--dump-outputs DIR``: after the timed steps, rank 0 writes what the last timed ``Environment.step``
+returned (observations, rewards, dones, infos) as ``DIR/<name>.npy`` (float32, or float64 for float64 and
+integer results), at most 64 MiB in all: above that, the same seeded sample of envs from every array
+(``DIR/sampled_envs.npy``).  Inputs depend only on the arguments, so two builds can be compared output
+for output.
+
+``--impl reference`` times the oracle port of the path (the reference is pure Python and is not
+part of this repository; the port issues the same eager torch op chain and is bit-identical to it,
 see tests/) through the same Environment API: on the host cores (default), or with
 ``--ref-device cuda`` on the GPU — the reference's own PyTorch-CUDA path.
 """
@@ -97,6 +103,7 @@ def parse_args():
     p.add_argument("--no-cpu-baseline", action="store_true")
     p.add_argument("--no-flush", action="store_true", help="keep L2 warm between iterations (not a bench value)")
     p.add_argument("--no-graph", action="store_true", help="step eagerly instead of replaying a CUDA graph")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's results as .npy")
     return p.parse_args()
 
 
@@ -108,7 +115,7 @@ def dist_info():
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     QUERY = (
         "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -169,6 +176,42 @@ class ClockSampler:
             "samples": len(sm),
             "reasons": sorted(reasons),
         }
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, result, limit=DUMP_LIMIT_BYTES):
+    """``result``: what ``Environment.step`` returned -> ``out_dir/<name>.npy``, one file per leaf tensor
+    (every leaf has the env batch as its first dimension)."""
+    import numpy as np
+
+    obs, rews, dones, infos = result
+    leaves = {}
+
+    def add(name, x):
+        if isinstance(x, dict):
+            for k in sorted(x):
+                add(f"{name}_{k}", x[k])
+        elif isinstance(x, (list, tuple)):
+            for i, v in enumerate(x):
+                add(f"{name}_{i}", v)
+        elif isinstance(x, torch.Tensor):
+            wide = x.dtype == torch.float64 or not (x.is_floating_point() or x.dtype == torch.bool)
+            leaves[name] = x.detach().to("cpu", torch.float64 if wide else torch.float32)
+
+    add("obs", obs), add("rew", rews), add("done", dones), add("info", infos)
+    total = sum(t.numel() * t.element_size() for t in leaves.values())
+    os.makedirs(out_dir, exist_ok=True)
+    if total > limit:  # a fixed, seeded sample of envs, the same rows of every array
+        batch = next(iter(leaves.values())).shape[0]
+        keep = max(1, batch * limit // total)
+        rows = np.sort(np.random.default_rng(0).choice(batch, size=keep, replace=False))
+        np.save(os.path.join(out_dir, "sampled_envs.npy"), rows.astype(np.float64))
+        leaves = {k: t[torch.from_numpy(rows)] for k, t in leaves.items()}
+    for name, t in leaves.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.numpy())
+    return sorted(leaves)
 
 
 def pregenerate_actions(env, steps, seed, device, pin=False):
@@ -334,8 +377,8 @@ def main_reference(args):
             "workload": workload_string(cfg, per_gpu, total, world, scaling),
             "reference_device": args.ref_device,
             "note": "oracle port of the reference path (the same eager torch op chain, bit-identical to the "
-            "reference on CPU, tests/test_oracle_vs_reference.py); the pure-Python reference does not travel "
-            "to the GPU box.  Each step is one GPU's share of the workload (env-steps/s does not depend on it)",
+            "reference on CPU, tests/test_oracle_vs_reference.py); the pure-Python reference is not part of "
+            "this repository.  Each step is one GPU's share of the workload (env-steps/s does not depend on it)",
         },
         "cpu_baseline": {
             "value": value,
@@ -393,8 +436,8 @@ def main_b200(args):
         torch.cuda.synchronize()
         if world > 1:
             dist.barrier()
-            # a rank that slept in the barrier runs its first step's host work slowly (first bracket 0.1-0.17 ms
-            # against a median of 0.03, profiles/r2_4gpu_bench.json): spin the core awake, outside every bracket
+            # a rank that slept in the barrier runs its first step's host work slowly: spin the core awake,
+            # outside every bracket
             t0 = time.perf_counter()
             while time.perf_counter() - t0 < 2e-3:
                 pass
@@ -403,28 +446,32 @@ def main_b200(args):
     def timed_loop(step_fn, n):
         """Σ over iterations of the CUDA-event time of step_fn(i); L2 flushed outside the brackets."""
         pairs = []
+        result = None
         for i in range(n):
             if flush is not None:
                 flush.zero_()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            step_fn(i)
+            result = step_fn(i)
             e1.record()
             pairs.append((e0, e1))
         torch.cuda.synchronize()
         times = [a.elapsed_time(b) for a, b in pairs]
         timed_loop.last = times
+        timed_loop.result = result  # what the last step returned
         return sum(times)  # ms
 
     remeasured = []
     counted = {"before": 0}  # backend.launches at the start of the pass that counts
 
     def measured(step_fn, n, label):
-        """timed_loop, once more if a bracket shows a transient stall of the box: > 4x the median and at least
-        0.05 ms above it.  Seen as one ~50 ms bracket in the middle of a loop (about one run in 15 on an otherwise
-        idle GPU) and as a 0.17 ms first bracket behind the multi-rank barrier (profiles/r2_4gpu_bench.json); the
-        brackets of an undisturbed loop stay within 1.4x of their median.  Reported in the line."""
+        """timed_loop, once more if a bracket shows a transient stall of the GPU: > 4x the median and at least
+        0.05 ms above it (a stall of another process's making, or the first bracket behind the multi-rank
+        barrier).  Reported in the line.  ``measured.result``: what the first pass's last step returned — a second
+        pass repeats the same actions from a later state, so only the first pass's results are the same from run
+        to run."""
         ms = timed_loop(step_fn, n)
+        measured.result = timed_loop.result
         times = sorted(timed_loop.last)
         if n >= 5 and times[-1] > 4 * times[len(times) // 2] and times[-1] > times[len(times) // 2] + 0.05:
             remeasured.append(
@@ -448,6 +495,7 @@ def main_b200(args):
     counted["before"] = backend.launches
     wall0 = time.perf_counter()
     ms_total = measured(lambda i: env.step(dev_actions[W + i]), K, "value")
+    last_result = measured.result
     wall = time.perf_counter() - wall0
     brackets = sorted(timed_loop.last)
     bracket_us = {
@@ -496,8 +544,7 @@ def main_b200(args):
     # one pinned block per step ([A, B, action_size] when the agents' actions have one size): one upload
     same_size = len({tuple(a.shape) for a in host_actions[0]}) == 1
     # Environment.step is handed the pinned host tensors themselves: the step's kernel reads them over PCIe where
-    # they lie (no staging copy).  Measured against an explicit upload in front of the step: 187 vs 208 us per
-    # step (profiles/r2z_bench_pinned.json, r2z_bench.json).  VMAS_BENCH_PINNED_ACTIONS=0: the explicit upload.
+    # they lie (no staging copy).  VMAS_BENCH_PINNED_ACTIONS=0: an explicit upload in front of the step.
     pinned_actions = os.environ.get("VMAS_BENCH_PINNED_ACTIONS", "1") == "1" and env.continuous_actions
     # one pinned block per step ([A, B, action_size] when the agents' actions have one size): one upload
     same_size = len({tuple(a.shape) for a in host_actions[0]}) == 1
@@ -506,8 +553,7 @@ def main_b200(args):
         dev_block = torch.empty_like(host_blocks[0], device=device)
     obs0, rew0, done0, _ = env.step(dev_actions[0])
     # pinned host buffers for a step's results (observations and rewards of all agents as one tensor each,
-    # dones), two sets: every separate download costs ~8 us of the bracket (measured: one copy per result
-    # tensor 231 us per step, three copies 205 us; profiles/r2y_bench_per_tensor_downloads.json)
+    # dones), two sets: every separate download adds its own latency to the bracket
     host_sets = [
         (
             torch.empty((len(obs0),) + tuple(obs0[0].shape), dtype=obs0[0].dtype).pin_memory(),
@@ -530,9 +576,9 @@ def main_b200(args):
 
     def e2e_step(i):
         main = torch.cuda.current_stream()
-        # this step's actions first (an explicit host->device copy issued while the 8 MB download is in flight
-        # crawls at ~5 GB/s and holds the step's first kernel back; profiles/r2f_e2e_timeline.txt), then the
-        # previous step's results start travelling while this step's kernels run
+        # this step's actions first (an explicit host->device copy issued while the download is in flight
+        # crawls and holds the step's first kernel back), then the previous step's results start travelling
+        # while this step's kernels run
         if pinned_actions:
             actions = host_actions[(W + i) % len(host_actions)]  # (read by the step's kernel where they lie)
         elif same_size:
@@ -553,7 +599,6 @@ def main_b200(args):
         torch.cuda.current_stream().wait_stream(copy_stream)
 
     # untimed warm-up of the pipelined loop: the first dozens of transfers after an idle link are slower
-    # (measured: 285 us per step over the first 20 steps, 205 us in steady state)
     for t in range(max(40, W)):
         e2e_step(t - W)
     barrier()
@@ -578,27 +623,14 @@ def main_b200(args):
         if world > 1:
             dist.destroy_process_group()
         return
+    dumped = dump_outputs(args.dump_outputs, last_result) if args.dump_outputs else None
 
     # ---- roofline of the fused substep kernel -----------------------------------------------------
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_path):
-        peak = float(json.load(open(peaks_path))["hbm_gbs"])
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
-    else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+    peak, peak_src = 3350.0, "NVIDIA H100 SXM data sheet (3.35 TB/s HBM3)"
     # one launch advances B envs by one substep (worlds with line / box pairs) or by all S substeps
     # (sphere-only worlds: the state stays in registers); bytes per launch = bytes x B either way
     alg_bytes = bytes_per_env_substep * B
     achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
-    traffic = traffic_src = None
-    tj = {}
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        ent = tj["%s_%s" % (cfg["scenario"], "_".join(f"{k}={v}" for k, v in cfg["kwargs"].items()))][str(B)]
-        traffic = ent["dram_bytes_read"] + ent["dram_bytes_write"]
-        traffic_src = ent["source"]
-    except Exception:  # noqa: BLE001
-        pass
     roofline = {
         "bound": "hbm",
         "kernel": "substep kernel, mapping=%s, arithmetic=%s" % (backend._dev_tables.mapping, nat.ARITH),
@@ -606,8 +638,6 @@ def main_b200(args):
         "peak": peak,
         "unit": "GB/s",
         "frac": achieved / peak,
-        "traffic": traffic,
-        "traffic_source": traffic_src,
         "peak_source": peak_src,
         "bytes_per_launch": alg_bytes,
         "bytes_per_env_substep": bytes_per_env_substep,
@@ -637,13 +667,6 @@ def main_b200(args):
         # Every timed step was ONE launch (step_env_kernel: action ingest + broad phase + substeps + step program
         # + observation rows): that kernel is the timed region, and the bracket around Environment.step is its
         # duration (plus the two event records).  The substep kernel on its own is kept below.
-        traffic = traffic_src = None
-        try:
-            ent = tj["%s_%s" % (cfg["scenario"], "_".join(f"{k}={v}" for k, v in cfg["kwargs"].items()))]["step_env_kernel"][str(B)]
-            traffic = ent["dram_bytes_read"] + ent["dram_bytes_write"]
-            traffic_src = ent["source"]
-        except Exception:  # noqa: BLE001
-            pass
         step_us = ms_total / K * 1e3
         roofline = {
             "bound": "hbm",
@@ -653,8 +676,6 @@ def main_b200(args):
             "peak": peak,
             "unit": "GB/s",
             "frac": step_bytes / (step_us * 1e-6) / 1e9 / peak,
-            "traffic": traffic,
-            "traffic_source": traffic_src,
             "peak_source": peak_src,
             "bytes_per_launch": step_bytes,
             "bytes_per_env_substep": bytes_per_env_substep,
@@ -774,8 +795,6 @@ def main_b200(args):
                 "max": round(1e3 * max(e2e_brackets), 1),
                 "largest": [[i, round(1e3 * x, 1)] for x, i in sorted(((x, i) for i, x in enumerate(e2e_brackets)), reverse=True)[:3]],
             },
-            "pcie_roofline": "the download alone (8.4 MB at the measured 56 GB/s, profiles/r2b_pcie.txt) is 160 us per "
-            "step of 32768 balance envs = 2.05e8 env-steps/s",
         },
         "gpu_launches": launches,
         "roofline": roofline,
@@ -783,6 +802,7 @@ def main_b200(args):
         "per_rank_ms_per_step": [float(r[0]) / K for r in per_rank],
         "per_rank_e2e_ms_per_step": [float(r[1]) / K for r in per_rank],
         "cpu_baseline": cpu_baseline,
+        "dumped_outputs": dumped,
     }
     print(json.dumps(line), flush=True)
     if world > 1:

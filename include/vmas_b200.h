@@ -1,9 +1,9 @@
 /*
- * vmas_b200.h — C ABI of the B200 (sm_100a) physics hot path of VMAS.
+ * vmas_b200.h — C ABI of the H100 (sm_90a) physics hot path of VMAS.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch types.  Every entry point
  * replaces one piece of the reference's pure-Python/PyTorch hot path
- * (/root/reference/vmas/simulator/core.py); the Python host (ctypes, see
+ * (vmas/simulator/core.py); the Python host (ctypes, see
  * vectorizedmultiagentsimulator_b200/_native.py and INTEGRATION.md) passes device pointers of
  * tensors it owns plus the CUDA stream to launch on.  Nothing here allocates device memory or
  * synchronises the device.
@@ -124,7 +124,7 @@ const char* vmas_b200_specialization_name(int index);
 /*
  * Run-time specialisation.  Any world can get the specialised kernels: the host generates the
  * world's constexpr tables (codegen.emit_world), compiles csrc/spec_kernel.cuh for them into a small
- * shared object (simulator/jit.py: nvcc for sm_100a, cached by world hash) and registers the object's
+ * shared object (simulator/jit.py: nvcc for sm_90a, cached by world hash) and registers the object's
  * launch functions here.  `launch` / `launch_tile`: addresses of
  *     cudaError_t fn(const vmas::SpecArgs&, cudaStream_t)      (launch_tile may be NULL)
  * `spec_args_bytes` = sizeof(vmas::SpecArgs) as the object was compiled (layout check).

@@ -1,10 +1,10 @@
-"""CPU ORACLE for the B200 physics hot path — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
+"""CPU ORACLE for the CUDA physics hot path — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
 A torch-fp32, CPU-only restatement of the reference's ``World.step``, LIDAR ray cast and
-distance queries (``/root/reference/vmas/simulator/{core,physics,joints}.py``), used as the
+distance queries (``vmas/simulator/{core,physics,joints}.py``), used as the
 checker the CUDA kernels are compared against.
 
-Parity status: PINNED — validated live against the unmodified reference in this container
+Parity status: PINNED — validated against the unmodified reference's recorded roll-outs
 (``tests/test_oracle_vs_reference.py``) and against committed golden roll-outs generated from
 the reference (``tests/golden/``, made by ``tests/make_golden.py``).
 

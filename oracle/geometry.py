@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure, not product code) — closest-point geometry on CPU.
 
 A plain torch-fp32 restatement of the reference's batched closest-point routines
-(``/root/reference/vmas/simulator/physics.py``).  Every function is shape-generic: it works
+(``vmas/simulator/physics.py``).  Every function is shape-generic: it works
 on one pair (``[B, 2]``) or on a whole stacked bucket (``[B, P, 2]`` with per-pair lengths
 ``[P, 1]``), which is how ``oracle/world_step.py`` calls it.  Every function cites the
 reference lines it follows.  Arithmetic order and fp32 scalar rounding follow the reference expression by

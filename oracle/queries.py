@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure, not product code) — LIDAR ray casting and distance queries on CPU.
 
 Torch-fp32 restatement of ``World.cast_rays`` and its three shape kernels
-(``/root/reference/vmas/simulator/core.py:1281-1372, 1414-1490, 1544-1626, 1662-1786``) and of
+(``vmas/simulator/core.py:1281-1372, 1414-1490, 1544-1626, 1662-1786``) and of
 ``get_distance_from_point`` / ``get_distance`` / ``is_overlapping`` (core.py:1788-1969).
 Pinned the same way as ``oracle/world_step.py`` (live reference comparison + golden fixtures).
 """

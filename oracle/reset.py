@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure, not product code) — episode reset on the CPU, in numpy.
 
 Restates the reference's respawn procedure
-(``/root/reference/vmas/simulator/utils.py:241-319`` ``ScenarioUtils.spawn_entities_randomly`` /
+(``vmas/simulator/utils.py:241-319`` ``ScenarioUtils.spawn_entities_randomly`` /
 ``find_random_pos_for_entity``: per entity, propose a uniform position in the bounds and re-draw it
 in the envs where it is closer than ``min_dist`` to an occupied position) and the state zeroing of
 ``World.reset`` (``core.py:1179-1181`` → ``EntityState._reset`` ``core.py:286-296``), with the

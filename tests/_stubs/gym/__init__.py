@@ -1,6 +1,5 @@
-"""Test-only stand-in for ``gym`` so the UNMODIFIED reference (``/root/reference``) imports in
-this container (it needs ``gym.Env`` and ``gym.spaces``; gym is not installed and there is no
-network).  Never imported by the product package."""
+"""Test-only stand-in for ``gym`` so the UNMODIFIED reference imports without
+gym installed (it needs ``gym.Env`` and ``gym.spaces``).  Never imported by the product package."""
 from . import spaces  # noqa: F401
 
 

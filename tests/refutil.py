@@ -1,15 +1,17 @@
-"""Test helpers to run the UNMODIFIED reference (read-only checkout) in this container."""
+"""Helpers of tests/make_golden.py to run the UNMODIFIED reference (a read-only checkout named by ``VMAS_REF``)."""
 import os
 import sys
 
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REFERENCE_DIR = os.environ.get("VMAS_REF", "/root/reference")
+REFERENCE_DIR = os.environ.get("VMAS_REF", "")
 
 
 def import_reference():
     """Imports the reference's ``vmas`` with the test-only ``gym`` stub on the path."""
+    if not os.path.isdir(os.path.join(REFERENCE_DIR, "vmas")):
+        raise RuntimeError("set VMAS_REF to a checkout of the reference VMAS (the directory holding vmas/)")
     stubs = os.path.join(HERE, "_stubs")
     for p in (REFERENCE_DIR, stubs):
         if p not in sys.path:

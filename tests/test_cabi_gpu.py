@@ -1,4 +1,4 @@
-"""Parity of the sm_100a kernels, called through the C ABI, against reference roll-outs.
+"""Parity of the sm_90a kernels, called through the C ABI, against reference roll-outs.
 
 Teacher-forced: every golden step's exact ``World.step`` input (state slab + processed action
 forces) is loaded on the GPU, ``vmas_b200_world_step`` runs once, and the result is compared
@@ -76,7 +76,7 @@ def _close(got, want, atol=ATOL):
 def test_world_step_vs_reference_golden(name):
     if _native.ARITH == "fast" and name == "crafted_clamps":
         # the reason the fast-arithmetic build is opt-in: torques over a small moment of inertia land at 1.2x
-        # the tolerance (profiles/r2c_parity_fast.txt, DESIGN.md section 6)
+        # the tolerance (DESIGN.md section 6)
         pytest.xfail("VMAS_B200_ARITH=fast leaves the 1e-4 contract on this world")
     fix, desc, tables = load(name)
     lib = _native.load()

@@ -514,8 +514,8 @@ def test_every_way_of_issuing_a_captured_step_gives_the_same_bits(monkeypatch):
 
 def test_one_kernel_step_falls_back_when_the_batch_does_not_fit_the_gpu_at_once():
     """The one-kernel step's broad phase needs a grid-wide barrier, hence every block resident; beyond that
-    (here: more envs than 148 SMs x 8 blocks x 64 threads) the same call issues ingest + whole-step kernel."""
-    n_envs = 148 * 8 * 64 + 4096
+    (here: more envs than the GPU's SMs x 8 blocks x 64 threads) the same call issues ingest + whole-step kernel."""
+    n_envs = torch.cuda.get_device_properties(0).multi_processor_count * 8 * 64 + 4096
     big = b200.make_env("balance", num_envs=n_envs, device="cuda", seed=0, cuda_graph=True, n_agents=4)
     eager = b200.make_env("balance", num_envs=n_envs, device="cuda", seed=0, n_agents=4)
     big.reset()

@@ -1,5 +1,5 @@
 """Run-time specialisation (vectorizedmultiagentsimulator_b200/jit.py) without a GPU: the world's tables are
-emitted, nvcc cross-compiles the object for sm_100a, its launch functions are registered with the
+emitted, nvcc cross-compiles the object for sm_90a, its launch functions are registered with the
 main library and the plan upload then selects the specialised mapping.  (Launching it is
 tests/test_cabi_gpu.py::test_runtime_specialisation_agrees_bitwise, on the GPU.)"""
 import pytest

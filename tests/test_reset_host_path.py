@@ -262,30 +262,3 @@ def test_shards_reset_like_the_unsharded_job(device_reset_on_cpu, name, kwargs):
         for (k, got), want in zip(_slab(part).items(), _slab(full).values()):
             assert torch.equal(got, want[lo:hi]), f"{name} rank {rank}: {k}"
 
-
-@pytest.mark.reference
-@pytest.mark.timeout(600)
-def test_reference_scenario_files_reset_through_the_device_path():
-    """Every UNMODIFIED scenario file of the reference: construction (first reset), ``reset_at(i)``
-    and ``reset()`` through the device-reset marshalling — whatever arguments they hand to
-    ``ScenarioUtils`` (occupied blocks per env or shared, goals drawn without an entity, respawns
-    in the middle of an episode) must be accepted, and resetting must not need the compiled plan
-    (``joint_passage``'s collision filter reads state its first reset creates).  Runs in its own
-    process: the scenario files import ``vmas``, which must resolve to this package's alias."""
-    import json
-    import os
-    import subprocess
-    import sys
-
-    here = os.path.dirname(os.path.abspath(__file__))
-    proc = subprocess.run(
-        [sys.executable, os.path.join(here, "reset_hostpath_runner.py")], capture_output=True, text=True, timeout=550
-    )
-    assert proc.returncode == 0, proc.stderr[-2000:]
-    report = json.loads(proc.stdout.strip().splitlines()[-1])
-    assert len(report) >= 40
-    failures = {k: v for k, v in report.items() if v.get("error")}
-    assert not failures, failures
-    for name, r in report.items():
-        assert r["spawn_failures"] == 0 and r["reset_count"] == [2, 2, 2, 3, 2], name
-    assert sum(r["spawn_calls"] > 0 for r in report.values()) >= 8  # the scenarios that use ScenarioUtils

@@ -1,6 +1,6 @@
 """env-steps/s of Environment.step (CUDA-graph mode) on the BASELINE.json configs C2-C5 at 1 GPU.
 
-    python tools/config_bench.py > profiles/r1_config_bench.jsonl
+    python tools/config_bench.py
 
 One JSON line per config: CUDA events around each step, 512 MiB L2 flush between steps (outside
 the events), actions resident on the device.  C5 is run at the per-GPU share of an 8-GPU job

@@ -1,10 +1,11 @@
 """How much can sorting envs by contact signature reduce a warp's divergent work?  (CPU study: real roll-out
 states from the oracle env, signatures from the specialised kernel's device code run on the host, tests/hostsim.)
 
-    python tools/grouping_study.py > profiles/r2_grouping_study.txt
+    python tools/grouping_study.py
 """
-import sys, ctypes as C, numpy as np, torch
-sys.path.insert(0,'/root/repo'); sys.path.insert(0,'/root/repo/tests')
+import os, sys, ctypes as C, numpy as np, torch
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import vectorizedmultiagentsimulator_b200 as b200
 from oracle.backend import use_oracle
 from vectorizedmultiagentsimulator_b200 import codegen

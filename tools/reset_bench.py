@@ -1,6 +1,6 @@
 """Cost of resetting finished envs (SURVEY §8(f)-4), on one GPU.
 
-    python tools/reset_bench.py > profiles/r1g_reset_bench.jsonl
+    python tools/reset_bench.py
 
 For each scenario: wall-clock (host + device, synchronised) of
   * ``reset_at(mask)`` with 25 % of the envs flagged — device-side reset (this library's kernels);

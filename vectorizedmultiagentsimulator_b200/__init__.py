@@ -1,7 +1,7 @@
-"""vectorizedmultiagentsimulator_b200 — a B200-native drop-in for VMAS's physics hot path.
+"""vectorizedmultiagentsimulator_b200 — an H100-native drop-in for VMAS's physics hot path.
 
 ``World.step`` (batched 2-D rigid-body substep: forces, Sphere/Box/Line contacts, joints,
-semi-implicit Euler) and the LIDAR ray cast are hand-written sm_100a CUDA kernels behind the
+semi-implicit Euler) and the LIDAR ray cast are hand-written sm_90a CUDA kernels behind the
 reference's own Python API (``make_env`` / ``Environment.step`` / ``BaseScenario``).
 """
 from .make_env import make_env

@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI library ``libvmas_b200.so`` (``include/vmas_b200.h``).
 
-The library is built in-tree by :func:`build` (``nvcc -gencode arch=compute_100a,code=sm_100a``)
+The library is built in-tree by :func:`build` (``nvcc -gencode arch=compute_90a,code=sm_90a``)
 and loaded by :func:`load`, which fails loudly if it is missing: there is no fallback path.
 PyTorch only provides device memory and the current stream; every kernel is this library's.
 """
@@ -54,10 +54,10 @@ ARITH_FLAGS = {
 }
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-O3",
     "-lineinfo",
-    "-DSPEC_MIN_BLOCKS=8",  # <= 128 registers for the specialised kernels: 16 warps/SM (measured best)
+    "-DSPEC_MIN_BLOCKS=8",  # <= 128 registers for the specialised kernels: 16 warps/SM
     "-std=c++17",
     "-Xcompiler",
     "-fPIC",
@@ -81,7 +81,7 @@ def needs_build(lib_path: Optional[str] = None) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, arith: Optional[str] = None) -> str:
-    """Compile the CUDA sources for sm_100a into ``libvmas_b200.so`` (``arith="fast"``:
+    """Compile the CUDA sources for sm_90a into ``libvmas_b200.so`` (``arith="fast"``:
     ``libvmas_b200_fast.so``) next to this file.  Default: the variant this process loads."""
     from . import codegen
 
@@ -193,7 +193,7 @@ GROUP_TILE = -8  # VMAS_GROUP_TILE
 #: env scheduling of the specialised thread-per-env kernel: the envs are re-sorted by their contact
 #: signature every this many World.step calls (0 = off: thread t always steps env t).  OFF by default:
 #: it halves the warp-instructions (1.8 k per 32 envs at 31 of 32 lanes active) but the scattered rows
-#: leave the kernel latency-bound — measured slower on real roll-out states (profiles/r2f_*)
+#: leave the kernel latency-bound — measured slower on real roll-out states
 ENV_REORDER_EVERY = int(os.environ.get("VMAS_B200_ENV_REORDER_EVERY", "0"))
 ENV_REORDER_MIN_BATCH = 1024  # below this there is nothing to gain from grouping
 ENV_REORDER_CHUNK = int(os.environ.get("VMAS_B200_ENV_REORDER_CHUNK", "2048"))  # envs sorted together
@@ -267,7 +267,7 @@ _lib = None
 
 
 def load():
-    """Load the built library (never builds implicitly on a GPU box: ship the ``.so``)."""
+    """Load the built library (never builds implicitly: run ``build()`` first)."""
     global _lib
     if _lib is not None:
         return _lib

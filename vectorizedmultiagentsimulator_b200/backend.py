@@ -96,7 +96,7 @@ def _require_cuda(world):
     dev = torch.device(world.device)
     if dev.type != "cuda":
         raise RuntimeError(
-            f"vectorizedmultiagentsimulator_b200 runs its physics only on CUDA (sm_100a); world device is "
+            f"vectorizedmultiagentsimulator_b200 runs its physics only on CUDA (sm_90a); world device is "
             f"'{dev}'. There is no CPU fallback."
         )
     if dev.index is None:  # "cuda" -> the concrete device its tensors live on
@@ -105,7 +105,7 @@ def _require_cuda(world):
 
 
 class CudaBackend(PlanRuntime):
-    """One process-local driver of the sm_100a kernels for one world (one GPU)."""
+    """One process-local driver of the sm_90a kernels for one world (one GPU)."""
 
     def __init__(self, world):
         super().__init__(world)

@@ -24,10 +24,9 @@ GENERATED = os.path.join(HERE, "csrc", "generated", "specializations.cuh")
 
 #: worlds that get an ahead-of-time specialisation: (scenario, kwargs[, tuning]).
 #: tuning["min_blocks"]: resident blocks per SM the register allocator leaves room for (default: the
-#: build's SPEC_MIN_BLOCKS = 8, i.e. <= 128 registers at 64 threads per block).  Measured per world
-#: on B200 (profiles/r1g_variant_bench.txt): stock transport runs 11 % faster at 1 Mi envs with 12
-#: (80 registers, 24 warps / SM) and the same at 32768; navigation loses 28 % there, balance and
-#: flocking gain 3-7 % at 1 Mi envs but lose 9-12 % at 32768, so they stay at the default.
+#: build's SPEC_MIN_BLOCKS = 8, i.e. <= 128 registers at 64 threads per block).  Chosen per world by
+#: measurement: stock transport with 12 (80 registers, 24 warps / SM), the others at the default (not yet
+#: re-measured on H100, which has the same 64 K registers per SM).
 PRESETS: List[Tuple] = [
     ("balance", dict(n_agents=4)),  # BASELINE.json configs[0], [1]
     ("balance", dict()),

@@ -42,7 +42,7 @@ _MODULES = [
 
 
 def _render_interactively(*args, **kwargs):
-    raise NotImplementedError("Interactive rendering is outside the scope of the B200 hot-path build")
+    raise NotImplementedError("Interactive rendering is outside the scope of the CUDA hot-path build")
 
 
 def install_vmas_alias(force: bool = False) -> None:

@@ -1,7 +1,7 @@
 // geometry.cuh — scalar (one pair, one env) narrow-phase geometry for the VMAS physics kernels.
 //
 // Each routine is the per-element arithmetic of one batched routine of the reference
-// (/root/reference/vmas/simulator/physics.py, cited per function), written for registers:
+// (vmas/simulator/physics.py, cited per function), written for registers:
 // segments carry their precomputed unit direction so sin/cos are evaluated once per entity per
 // substep.  The file is compiled with -fmad=false: every multiply and add rounds separately,
 // like the reference's chain of eager elementwise ops; the only fused operation is inside
@@ -34,7 +34,7 @@ DEVI float sgnf(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }  // 
 // is zero (FCHK fails), which is the common case here (contact normals along an axis, resting bodies,
 // zero torque) — and a select does not help: the compiler evaluates the division for every lane and
 // the lanes with a zero numerator still walk the slow path (measured: 14 % of the balance kernel's
-// warp-instructions, profiles/r2a_*).  So the division itself is given a harmless numerator (1) in
+// warp-instructions).  So the division itself is given a harmless numerator (1) in
 // that case; (+-0) / b == +-0 for b > 0, so the numerator itself is the exact quotient.
 DEVI float div_pos(float a, float b) {
   const bool zero = (a == 0.f && b > 0.f);

@@ -5,7 +5,7 @@
 // part of an item (is the pair anywhere near contact?) is uniform, but the expensive part (closest
 // points of boxes / segments, the soft-plus contact force with its IEEE divisions, expf, log1pf) is
 // needed by a different subset of items in every env: a warp executes it once per item that is near
-// in ANY of its 32 envs, with ~8 of 32 lanes active (ncu, profiles/r2a_*: 60 % of the balance
+// in ANY of its 32 envs, with ~8 of 32 lanes active (ncu: 60 % of the balance
 // kernel's warp-instructions run at 5-13 lanes).
 //
 // Here a warp owns a tile of 32 envs.  Per substep:

@@ -1,4 +1,4 @@
-// vmas_b200.cu — sm_100a kernels + C ABI for the VMAS physics hot path (see include/vmas_b200.h).
+// vmas_b200.cu — sm_90a kernels + C ABI for the VMAS physics hot path (see include/vmas_b200.h).
 //
 // Kernels
 //   step_kernel<G, EPL>   fused substep(s): per-entity forces -> joint/contact work items ->
@@ -13,7 +13,7 @@
 //   pair_query_kernel /   World.get_distance / is_overlapping / get_distance_from_point.
 //   point_query_kernel
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false (no fast-math).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (no fast-math).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -2443,7 +2443,7 @@ int vmas_b200_copy_buffers(const VmasCopySegment* segs, int32_t n_segs, void* cu
     a.seg[i] = segs[i];
     a.first_block[i] = blocks;
     size_t want = (segs[i].bytes + per_block - 1) / per_block;
-    want = want < 1 ? 1 : (want > 148 * 8 ? 148 * 8 : want);
+    want = want < 1 ? 1 : (want > 132 * 8 ? 132 * 8 : want);  // at most 8 blocks per SM of an H100 SXM
     blocks += (int)want;
   }
   a.first_block[n_segs] = blocks;

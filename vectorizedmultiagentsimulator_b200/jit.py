@@ -5,7 +5,7 @@ are the reference's contract).
 to run on the generic table-driven kernels at 2-15x the time.  Here the same template
 (``csrc/spec_kernel.cuh``) is compiled for the world at hand when its plan is first uploaded: the
 world's constexpr tables are emitted (``codegen.emit_world``), ``nvcc`` builds a small shared object
-for sm_100a (a few seconds, in a background thread; cached on disk by world hash and arithmetic
+for sm_90a (a few seconds, in a background thread; cached on disk by world hash and arithmetic
 flags), and its launch functions are registered with the main library
 (``vmas_b200_register_specialization``).  Until the object is ready the world steps on the generic
 kernels; both produce identical bits (tests/test_cabi_gpu.py), so the switch is invisible.
@@ -18,6 +18,7 @@ import ctypes as C
 import hashlib
 import os
 import subprocess
+import tempfile
 import threading
 from typing import Dict, Optional
 
@@ -26,7 +27,10 @@ from .simulator import plan as P
 
 MODE = os.environ.get("VMAS_B200_JIT", "async")
 assert MODE in ("async", "block", "off"), MODE
-CACHE_DIR = os.environ.get("VMAS_B200_JIT_DIR") or os.path.join(_native.CSRC, "generated", "jit")
+#: the objects ``__graft_entry__.build`` compiles (``prebuild_step_kernels``) ship in the package tree
+PREBUILT_DIR = os.path.join(_native.CSRC, "generated", "jit")
+#: what a run compiles goes to a per-user directory outside the tree, which may be read-only
+CACHE_DIR = os.environ.get("VMAS_B200_JIT_DIR") or os.path.join(tempfile.gettempdir(), f"vmas_b200_jit_{os.getuid()}")
 
 _TEMPLATE = """// GENERATED at run time by vectorizedmultiagentsimulator_b200/jit.py — one world's specialised kernels.
 #include "spec_kernel.cuh"
@@ -89,12 +93,33 @@ def _source_stamp() -> str:
     return h.hexdigest()[:12]
 
 
+def _shared_object(stem: str, source: str, out_dir: str) -> str:
+    """Path of the object ``stem.so``: the prebuilt one, the cached one, or compiled from ``source`` into ``out_dir``."""
+    for d in (PREBUILT_DIR, CACHE_DIR, out_dir):
+        so = os.path.join(d, stem + ".so")
+        if os.path.exists(so):
+            return so
+    os.makedirs(out_dir, mode=0o700, exist_ok=True)
+    path = os.path.join(out_dir, stem)
+    with open(path + ".cu", "w") as fh:
+        fh.write(source)
+    flags = _native.NVCC_FLAGS + _native.ARITH_FLAGS[_native.ARITH]
+    tmp = f"{path}.so.{os.getpid()}.tmp"
+    cmd = [_native._nvcc()] + flags + ["-I", _native.INCLUDE, "-I", _native.CSRC, "-o", tmp, path + ".cu"]
+    proc = subprocess.run(cmd, capture_output=True, text=True)
+    if proc.returncode != 0:
+        raise RuntimeError(f"nvcc failed: {proc.stderr[-600:]}")
+    os.replace(tmp, path + ".so")  # atomic: concurrent processes (one per GPU) may race on the same world
+    return path + ".so"
+
+
 class Job:
     """One world's compilation: ``index`` is the registered specialisation once ``done`` is set."""
 
-    def __init__(self, desc: P.WorldDescription):
+    def __init__(self, desc: P.WorldDescription, out_dir: Optional[str] = None):
         self.hash = codegen.world_hash(desc)
         self.desc = desc
+        self.out_dir = out_dir or CACHE_DIR  # where the object is compiled to if no cache has it
         self.done = threading.Event()
         self.index = -1
         self.error: Optional[str] = None
@@ -114,20 +139,8 @@ class Job:
     def _compile_and_register(self) -> int:
         desc = self.desc
         name, text, h = codegen.emit_world(desc, "run-time specialisation")
-        os.makedirs(CACHE_DIR, exist_ok=True)
-        stem = os.path.join(CACHE_DIR, f"{h:016x}_{_native.ARITH}_{_source_stamp()}")
-        so = stem + ".so"
-        if not os.path.exists(so):
-            with open(stem + ".cu", "w") as fh:
-                fh.write(_TEMPLATE.format(world=text, name=name))
-            flags = _native.NVCC_FLAGS + _native.ARITH_FLAGS[_native.ARITH]
-            tmp = f"{so}.{os.getpid()}.tmp"
-            cmd = [_native._nvcc()] + flags + ["-I", _native.INCLUDE, "-I", _native.CSRC, "-o", tmp, stem + ".cu"]
-            proc = subprocess.run(cmd, capture_output=True, text=True)
-            if proc.returncode != 0:
-                raise RuntimeError(f"nvcc failed: {proc.stderr[-600:]}")
-            os.replace(tmp, so)  # atomic: concurrent processes (one per GPU) may race on the same world
-        obj = C.CDLL(so)
+        stem = f"{h:016x}_{_native.ARITH}_{_source_stamp()}"
+        obj = C.CDLL(_shared_object(stem, _TEMPLATE.format(world=text, name=name), self.out_dir))
         lib = _native.load()
         launch = C.cast(obj.vmas_jit_launch, C.c_void_p)
         tile = C.cast(obj.vmas_jit_launch_tile, C.c_void_p) if obj.vmas_jit_has_tile() else None
@@ -177,8 +190,8 @@ class StepKernelJob(Job):
     """The whole-step kernel of one (world, observation columns, step program): ``index`` is the handle for
     ``VmasEnvStep.fused_kernel`` once ``done`` is set."""
 
-    def __init__(self, desc: P.WorldDescription, cols, instrs, acts=()):
-        super().__init__(desc)
+    def __init__(self, desc: P.WorldDescription, cols, instrs, acts=(), out_dir: Optional[str] = None):
+        super().__init__(desc, out_dir)
         self.cols, self.instrs, self.acts = cols, instrs, tuple(acts)
         self.post_hash = codegen.post_hash(cols, instrs, self.acts)
         self.key = (self.hash ^ ((self.post_hash << 1) | (self.post_hash >> 63))) & 0xFFFFFFFFFFFFFFFF
@@ -187,20 +200,9 @@ class StepKernelJob(Job):
         desc = self.desc
         name, text, h = codegen.emit_world(desc, "whole-step kernel")
         post_name, post_text, _ = codegen.emit_post(self.cols, self.instrs, self.acts)
-        os.makedirs(CACHE_DIR, exist_ok=True)
-        stem = os.path.join(CACHE_DIR, f"step_{self.key:016x}_{_native.ARITH}_{_source_stamp()}")
-        so = stem + ".so"
-        if not os.path.exists(so):
-            with open(stem + ".cu", "w") as fh:
-                fh.write(_STEP_TEMPLATE.format(world=text, post=post_text, name=name, post_name=post_name))
-            flags = _native.NVCC_FLAGS + _native.ARITH_FLAGS[_native.ARITH]
-            tmp = f"{so}.{os.getpid()}.tmp"
-            cmd = [_native._nvcc()] + flags + ["-I", _native.INCLUDE, "-I", _native.CSRC, "-o", tmp, stem + ".cu"]
-            proc = subprocess.run(cmd, capture_output=True, text=True)
-            if proc.returncode != 0:
-                raise RuntimeError(f"nvcc failed: {proc.stderr[-600:]}")
-            os.replace(tmp, so)
-        obj = C.CDLL(so)
+        stem = f"step_{self.key:016x}_{_native.ARITH}_{_source_stamp()}"
+        source = _STEP_TEMPLATE.format(world=text, post=post_text, name=name, post_name=post_name)
+        obj = C.CDLL(_shared_object(stem, source, self.out_dir))
         lib = _native.load()
         with _lock:
             handle = lib.vmas_b200_register_step_kernel(
@@ -241,7 +243,7 @@ def request_step_kernel(desc: P.WorldDescription, cols, instrs, acts=(), block: 
 
 def prebuild_step_kernels(verbose: bool = False):
     """Compiles the whole-step kernels of the preset worlds (``codegen.PRESETS``) whose scenario is written
-    on a step program, so that they are in the on-disk cache before the first capture (``__graft_entry__.build``).
+    on a step program into ``PREBUILT_DIR``, so that they are there before the first capture (``__graft_entry__.build``).
     Returns ``[(label, key)]``."""
     import torch
 
@@ -249,10 +251,10 @@ def prebuild_step_kernels(verbose: bool = False):
 
     built = []
     stamp = f"_{_source_stamp()}."
-    if os.path.isdir(CACHE_DIR):  # objects compiled from older headers can never be loaded again
-        for name in os.listdir(CACHE_DIR):
+    if os.path.isdir(PREBUILT_DIR):  # objects compiled from older headers can never be loaded again
+        for name in os.listdir(PREBUILT_DIR):
             if stamp not in name:
-                os.remove(os.path.join(CACHE_DIR, name))
+                os.remove(os.path.join(PREBUILT_DIR, name))
     for scenario, kwargs, *_ in codegen.PRESETS:
         sc = scenarios.load(scenario + ".py").Scenario()
         if not (hasattr(sc, "_step_program") and hasattr(sc, "_observation_plan")):
@@ -283,7 +285,7 @@ def prebuild_step_kernels(verbose: bool = False):
             for a in agents
         ) if holonomic else ()
         for variant in ((), acts) if acts else ((),):
-            job = StepKernelJob(desc, columns, instrs, variant)
+            job = StepKernelJob(desc, columns, instrs, variant, out_dir=PREBUILT_DIR)
             job.run()
             if job.error:
                 raise RuntimeError(f"whole-step kernel of {label}: {job.error}")

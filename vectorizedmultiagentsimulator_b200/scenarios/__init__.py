@@ -1,6 +1,6 @@
 """Scenario lookup by file name (ref vmas/scenarios/__init__.py:11-24).
 
-Search order: this directory (the scenarios re-written for the B200 build), then every
+Search order: this directory (the scenarios re-written for the CUDA build), then every
 directory listed in ``$VMAS_SCENARIO_PATH`` (``os.pathsep``-separated; walked recursively), so
 an unmodified reference checkout's scenario files can be dropped in.  Files from outside this
 package import ``vmas.simulator...``; :func:`..compat.install_vmas_alias` is called so those

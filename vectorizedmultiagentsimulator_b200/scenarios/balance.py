@@ -2,7 +2,7 @@
 
 Task definition of the reference's ``vmas/scenarios/balance.py`` (world :17-84, reset :86-213,
 reward :220-239, observation :241-257, done :259-263) re-written on the public API for the
-B200 build: same entities, constants, random-draw order, observation layout and reward, but
+CUDA build: same entities, constants, random-draw order, observation layout and reward, but
 no host synchronisation in ``reward`` (masked assignment → ``torch.where``) and the three
 overlap tests are single kernel launches.
 """

@@ -42,7 +42,7 @@ class Scenario(BaseScenario):
         self.package_width = kwargs.pop("package_width", 0.15)
         self.package_length = kwargs.pop("package_length", 0.15)
         self.package_mass = kwargs.pop("package_mass", 50)
-        self.n_lines = kwargs.pop("n_lines", 0)  # B200-bench variant only
+        self.n_lines = kwargs.pop("n_lines", 0)  # bench.py variant only
         self.line_length = kwargs.pop("line_length", 0.3)
         substeps = kwargs.pop("substeps", 1)
         ScenarioUtils.check_kwargs_consumed(kwargs)

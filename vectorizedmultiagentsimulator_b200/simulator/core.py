@@ -8,7 +8,7 @@ Python:
 * state lives in a contiguous :class:`~.slab.StateSlab`; ``entity.state.pos`` & co. are
   writable views into it, and their setters copy *into* the slab;
 * ``World.step`` / ``cast_rays`` / ``get_distance`` / ``is_overlapping`` are single calls
-  into the sm_100a kernels through the C-ABI library (``include/vmas_b200.h``).  There is no
+  into the sm_90a kernels through the C-ABI library (``include/vmas_b200.h``).  There is no
   torch-eager or CPU implementation of the physics in this package: on a non-CUDA device, or
   without the built library, those calls raise.
 
@@ -95,7 +95,7 @@ class Shape(ABC):
         raise NotImplementedError
 
     def get_geometry(self):
-        raise NotImplementedError("Rendering is outside the scope of the B200 hot-path build")
+        raise NotImplementedError("Rendering is outside the scope of the CUDA hot-path build")
 
 
 class Box(Shape):
@@ -640,7 +640,7 @@ class Entity(TorchVectorizedObject, Observable, ABC):
         self.state.to(device)
 
     def render(self, env_index: int = 0):
-        raise NotImplementedError("Rendering is outside the scope of the B200 hot-path build")
+        raise NotImplementedError("Rendering is outside the scope of the CUDA hot-path build")
 
 
 class Landmark(Entity):
@@ -900,7 +900,7 @@ class Agent(Entity):
 # World (ref core.py:1090-2919)
 # ----------------------------------------------------------------------------------------
 class World(TorchVectorizedObject):
-    """Batched 2-D world whose ``step`` is one call into the B200 physics kernels.
+    """Batched 2-D world whose ``step`` is one call into the CUDA physics kernels.
 
     Constructor arguments are the reference's (ref core.py:1091-1108).  Two extra keyword
     arguments exist only here: ``check_scripted_actions`` (keep the reference's range assert

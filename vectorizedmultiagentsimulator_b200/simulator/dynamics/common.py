@@ -39,7 +39,7 @@ class Dynamics(abc.ABC):
         """Called on ``world.reset(index)``; stateless models have nothing to do."""
 
     def zero_grad(self):
-        """Kept for API compatibility; the B200 path carries no autograd graph."""
+        """Kept for API compatibility; the CUDA path carries no autograd graph."""
 
     # -- the contract ---------------------------------------------------------------------------
     @property

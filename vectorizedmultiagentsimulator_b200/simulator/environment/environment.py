@@ -97,8 +97,8 @@ def _seeded(method):
     return wrapper
 
 
-# opt-in (VMAS_B200_FORK_OBS=1): measured 5-8 % SLOWER on balance / navigation / flocking at the BASELINE
-# batch sizes (profiles/r2h_fork_ab.txt) — the branches of the captured graph do not start together
+# opt-in (VMAS_B200_FORK_OBS=1): measured slower on balance / navigation / flocking at the BASELINE
+# batch sizes — the branches of the captured graph do not start together
 _FORK_OBSERVATIONS = os.environ.get("VMAS_B200_FORK_OBS", "0") == "1"
 
 
@@ -141,7 +141,7 @@ class Environment(TorchVectorizedObject):
             ), "When asking for multidiscrete_actions, make sure continuous_actions=False"
         if grad_enabled:
             raise NotImplementedError(
-                "grad_enabled=True is not supported: the B200 physics kernels are forward-only"
+                "grad_enabled=True is not supported: the CUDA physics kernels are forward-only"
             )
         with local_seed(Environment.vmas_random_state):
             self.scenario = scenario
@@ -1272,7 +1272,7 @@ class Environment(TorchVectorizedObject):
     # ------------------------------------------------------------------------------------
     def render(self, *args, **kwargs):
         raise NotImplementedError(
-            "Rendering (pyglet viewer) is outside the scope of the B200 hot-path build"
+            "Rendering (pyglet viewer) is outside the scope of the CUDA hot-path build"
         )
 
     def to(self, device: DEVICE_TYPING):

@@ -184,4 +184,4 @@ class JointConstraint:
         return entity.state.pos + self.get_delta_anchor(entity)
 
     def render(self, env_index: int = 0):
-        raise NotImplementedError("Rendering is outside the scope of the B200 hot-path build")
+        raise NotImplementedError("Rendering is outside the scope of the CUDA hot-path build")

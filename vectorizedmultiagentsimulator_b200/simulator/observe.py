@@ -1,7 +1,7 @@
 """Observation blocks: every agent's observation assembled on the device in one or two launches.
 
 The reference builds an observation per agent from slices and ``torch.cat``
-(``/root/reference/vmas/scenarios/balance.py:236-262``, ``navigation.py:252-265``,
+(``vmas/scenarios/balance.py:236-262``, ``navigation.py:252-265``,
 ``flocking.py:186-199``): a dozen tiny kernels per agent per step.  Here a scenario describes its
 observation once as rows of *terms*; the world compiles the rows into a column table and
 ``World.observe(plan)`` fills the whole ``[rows, batch_dim, width]`` block with

@@ -88,7 +88,7 @@ def _shape_kind(shape) -> int:
         return SHAPE_BOX
     if name == "Line":
         return SHAPE_LINE
-    raise RuntimeError(f"Shape {shape} is not supported by the B200 physics kernels")
+    raise RuntimeError(f"Shape {shape} is not supported by the CUDA physics kernels")
 
 
 def _is_agent(entity) -> bool:
@@ -166,7 +166,7 @@ def describe_entity(entity, agent_index: int) -> Dict:
         v = getattr(entity, attr, None)
         if v is not None and not isinstance(v, (int, float)):
             raise NotImplementedError(
-                f"Entity '{entity.name}' has a tensor-valued {attr}; the B200 kernels take a scalar"
+                f"Entity '{entity.name}' has a tensor-valued {attr}; the CUDA kernels take a scalar"
             )
 
     def opt(name):

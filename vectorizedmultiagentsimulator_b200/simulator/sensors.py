@@ -8,7 +8,7 @@ import torch
 
 from .utils import Color
 
-_NO_RENDERING = "Rendering is outside the scope of the B200 hot-path build"
+_NO_RENDERING = "Rendering is outside the scope of the CUDA hot-path build"
 
 
 class Sensor(ABC):
