@@ -96,6 +96,12 @@ DEVI bool spec_far_apart(V2 a, V2 b, float reach) {
   return d.x * d.x + d.y * d.y > lim * lim;
 }
 
+// (x + y) + z with each sum rounded to float, as the kernel's run-time expressions round it
+__host__ __device__ constexpr float spec_add3(float x, float y, float z) {
+  const float s = x + y;
+  return s + z;
+}
+
 // Register-resident state of one env.
 template <int E>
 struct EnvRegs {
@@ -121,34 +127,86 @@ DEVI BoxG spec_box(const EnvRegs<E>& r) {
   return b;
 }
 
-// One work item, fully resolved at compile time; accumulates into the env's force registers in
-// the reference's order (ref core.py:2191-2199).
-// TRACK: also record in `sig` whether the item produced a force (env scheduling; off in the default kernel)
-template <class W, int I, bool TRACK, int E>
-DEVI void spec_item(EnvRegs<E>& r, const SpecArgs& a, long env, const uint32_t* mask_words, uint32_t& sig) {
-  constexpr ItemC it = W::item[I];
-  constexpr int A = it.a, B = it.b;
-  constexpr EntC ea = W::ent[A], eb = W::ent[B];
+// What one work item contributes: the force on `a` (`b` gets its negation) and the two torques
+struct ItemOut {
+  V2 f;
+  float ta, tb;
+};
+
+// Two items run the same code (and may share a round of the lane-pair step, see SpecRounds): same kind, same
+// mask gating, same joint rotation rule, same hollow flags.  Everything else differs only in constants.
+template <class W>
+__host__ __device__ constexpr bool spec_same_code(int i, int j) {
+  const ItemC x = W::item[i], y = W::item[j];
+  return x.kind == y.kind && (x.mask_bit >= 0) == (y.mask_bit >= 0) &&
+         (x.flags & VMAS_IFLAG_JOINT_ROTATE) == (y.flags & VMAS_IFLAG_JOINT_ROTATE) &&
+         (W::ent[x.a].flags & VMAS_F_HOLLOW) == (W::ent[y.a].flags & VMAS_F_HOLLOW) &&
+         (W::ent[x.b].flags & VMAS_F_HOLLOW) == (W::ent[y.b].flags & VMAS_F_HOLLOW);
+}
+
+// One work item's contribution, fully resolved at compile time (ref core.py:2191-2199).  Item I0 on an even
+// lane, I1 on an odd one (`odd`): the two must run the same code (spec_same_code), their entity indices and
+// constants are picked by selects on the lane's parity, never by a run-time index into the register arrays.
+// I0 == I1 (one lane per env, or a lone item): the selects fold away.
+template <class W, int I0, int I1, int E>
+DEVI ItemOut spec_item_eval(const EnvRegs<E>& r, const SpecArgs& a, long env, const bool odd) {
+  static_assert(I0 == I1 || spec_same_code<W>(I0, I1), "the items of a round must run the same code");
+  constexpr ItemC it = W::item[I0], jt = W::item[I1];
+  constexpr int A0 = it.a, B0 = it.b, A1 = jt.a, B1 = jt.b;
+  constexpr EntC ea = W::ent[A0], eb = W::ent[B0];  // (only their HOLLOW flags select code: same for both items)
   constexpr CfgC cfg = W::cfg;
-  if constexpr (it.mask_bit >= 0) {
-    if (a.use_mask && !((mask_words[it.mask_bit >> 5] >> (it.mask_bit & 31)) & 1u)) return;
-  }
+  const bool o = I0 != I1 && odd;
+  auto sel = [o](float x, float y) { return o ? y : x; };
+  const float dmin = sel(it.dmin_base, jt.dmin_base);
   V2 f = mk(0.f, 0.f);
   float ta = 0.f, tb = 0.f;
-  const V2 pa = mk(r.px[A], r.py[A]), pb = mk(r.px[B], r.py[B]);
+  const V2 pa = mk(sel(r.px[A0], r.px[A1]), sel(r.py[A0], r.py[A1]));
+  const V2 pb = mk(sel(r.px[B0], r.px[B1]), sel(r.py[B0], r.py[B1]));
+  const float ca = sel(r.c[A0], r.c[A1]), sa = sel(r.s[A0], r.s[A1]);
+  const float cb = sel(r.c[B0], r.c[B1]), sb = sel(r.s[B0], r.s[B1]);
+  auto seg_a = [&]() { return mkseg(pa, ca, sa, sel(W::ent[A0].d0 / 2.f, W::ent[A1].d0 / 2.f)); };
+  auto seg_b = [&]() { return mkseg(pb, cb, sb, sel(W::ent[B0].d0 / 2.f, W::ent[B1].d0 / 2.f)); };
+  auto box_a = [&]() {
+    BoxG b;
+    b.p = pa;
+    b.c = ca;
+    b.s = sa;
+    b.c2 = sel(r.c2[A0], r.c2[A1]);
+    b.s2 = sel(r.s2[A0], r.s2[A1]);
+    b.half_l = sel(W::ent[A0].d0 / 2.f, W::ent[A1].d0 / 2.f);
+    b.half_w = sel(W::ent[A0].d1 / 2.f, W::ent[A1].d1 / 2.f);
+    return b;
+  };
+  auto box_b = [&]() {
+    BoxG b;
+    b.p = pb;
+    b.c = cb;
+    b.s = sb;
+    b.c2 = sel(r.c2[B0], r.c2[B1]);
+    b.s2 = sel(r.s2[B0], r.s2[B1]);
+    b.half_l = sel(W::ent[B0].d0 / 2.f, W::ent[B1].d0 / 2.f);
+    b.half_w = sel(W::ent[B0].d1 / 2.f, W::ent[B1].d1 / 2.f);
+    return b;
+  };
+  // the far-test bounds (half extent of `a` + dmin) + margin, folded per item
+  constexpr float LIM_L0 = spec_add3(W::ent[A0].d0 / 2.f, it.dmin_base, SPEC_FAR_MARGIN);
+  constexpr float LIM_L1 = spec_add3(W::ent[A1].d0 / 2.f, jt.dmin_base, SPEC_FAR_MARGIN);
+  constexpr float LIM_W0 = spec_add3(W::ent[A0].d1 / 2.f, it.dmin_base, SPEC_FAR_MARGIN);
+  constexpr float LIM_W1 = spec_add3(W::ent[A1].d1 / 2.f, jt.dmin_base, SPEC_FAR_MARGIN);
 
   if constexpr (it.kind == VMAS_K_JOINT) {
-    V2 qa = pa + rot2(mk(it.ax, it.ay), r.c[A], r.s[A]);
-    V2 qb = pb + rot2(mk(it.bx, it.by), r.c[B], r.s[B]);
-    V2 f_attr = constraint_force(qa, qb, it.dist, cfg.joint_force, cfg.contact_margin, true);
-    V2 f_rep = constraint_force(qa, qb, it.dist, cfg.joint_force, cfg.contact_margin, false);
+    V2 qa = pa + rot2(mk(sel(it.ax, jt.ax), sel(it.ay, jt.ay)), ca, sa);
+    V2 qb = pb + rot2(mk(sel(it.bx, jt.bx), sel(it.by, jt.by)), cb, sb);
+    const float dist = sel(it.dist, jt.dist);
+    V2 f_attr = constraint_force(qa, qb, dist, cfg.joint_force, cfg.contact_margin, true);
+    V2 f_rep = constraint_force(qa, qb, dist, cfg.joint_force, cfg.contact_margin, false);
     f = f_attr + f_rep;
     V2 fb = neg(f_attr) + neg(f_rep);
     ta = cross2(qa - pa, f);
     tb = cross2(qb - pb, fb);
     if constexpr (!(it.flags & VMAS_IFLAG_JOINT_ROTATE)) {
-      float jr = a.joint_rot ? a.joint_rot[(size_t)env * W::N_JOINTS + I] : it.fixed_rot;
-      float delta = r.rot[A] - (r.rot[B] + jr);
+      float jr = a.joint_rot ? a.joint_rot[(size_t)env * W::N_JOINTS + (o ? I1 : I0)] : sel(it.fixed_rot, jt.fixed_rot);
+      float delta = sel(r.rot[A0], r.rot[A1]) - (sel(r.rot[B0], r.rot[B1]) + jr);
       float mag = sqrtf(delta * delta);
       float t = (cfg.torque_constraint_force * sgnf(delta)) * (expf(mag) - 1.f);
       if (mag < 1e-9f) t = 0.f;
@@ -156,81 +214,210 @@ DEVI void spec_item(EnvRegs<E>& r, const SpecArgs& a, long env, const uint32_t* 
       tb = tb + t;
     }
   } else if constexpr (it.kind == VMAS_K_SS) {
-    f = constraint_force(pa, pb, it.dmin_base, cfg.collision_force, cfg.contact_margin, false);
+    f = constraint_force(pa, pb, dmin, cfg.collision_force, cfg.contact_margin, false);
   } else if constexpr (it.kind == VMAS_K_LS) {  // a = line, b = sphere
-    Seg l = spec_seg<W, A>(r);
-    if (!spec_far_apart(l.p, pb, l.half + it.dmin_base)) {
+    Seg l = seg_a();
+    const V2 d = l.p - pb;
+    const float lim = sel(LIM_L0, LIM_L1);
+    if (!(d.x * d.x + d.y * d.y > lim * lim)) {  // (spec_far_apart)
       V2 cp = closest_point_seg(l, pb);
-      V2 f_sphere = constraint_force(pb, cp, it.dmin_base, cfg.collision_force, cfg.contact_margin, false);
+      V2 f_sphere = constraint_force(pb, cp, dmin, cfg.collision_force, cfg.contact_margin, false);
       f = neg(f_sphere);
       ta = cross2(cp - l.p, f);
     }
   } else if constexpr (it.kind == VMAS_K_LL) {
-    Seg l1 = spec_seg<W, A>(r), l2 = spec_seg<W, B>(r);
-    if (!spec_far_apart(l1.p, l2.p, l1.half + l2.half + it.dmin_base)) {
+    Seg l1 = seg_a(), l2 = seg_b();
+    if (!spec_far_apart(l1.p, l2.p, l1.half + l2.half + dmin)) {
       Pair c = closest_seg_seg(l1, l2);
-      f = constraint_force(c.a, c.b, it.dmin_base, cfg.collision_force, cfg.contact_margin, false);
+      f = constraint_force(c.a, c.b, dmin, cfg.collision_force, cfg.contact_margin, false);
       ta = cross2(c.a - l1.p, f);
       tb = cross2(c.b - l2.p, neg(f));
     }
   } else if constexpr (it.kind == VMAS_K_BS) {  // a = box, b = sphere
-    BoxG bx = spec_box<W, A>(r);
+    BoxG bx = box_a();
     V2 d0 = pb - bx.p;
     float lx = d0.x * bx.c + d0.y * bx.s, ly = d0.y * bx.c - d0.x * bx.s;
-    if (!(fabsf(lx) > bx.half_l + it.dmin_base + SPEC_FAR_MARGIN ||
-          fabsf(ly) > bx.half_w + it.dmin_base + SPEC_FAR_MARGIN)) {
+    if (!(fabsf(lx) > sel(LIM_L0, LIM_L1) || fabsf(ly) > sel(LIM_W0, LIM_W1))) {
       V2 cp = closest_point_box(bx, pb);
       V2 inner = cp;
       float d = 0.f;
       if constexpr (!(ea.flags & VMAS_F_HOLLOW)) inner = inner_point_box(pb, cp, bx.p, &d);
-      V2 f_sphere =
-          constraint_force(pb, inner, it.dmin_base + d, cfg.collision_force, cfg.contact_margin, false);
+      V2 f_sphere = constraint_force(pb, inner, dmin + d, cfg.collision_force, cfg.contact_margin, false);
       f = neg(f_sphere);
       ta = cross2(cp - bx.p, f);
     }
   } else if constexpr (it.kind == VMAS_K_BL) {  // a = box, b = line
-    BoxG bx = spec_box<W, A>(r);
-    Seg l = spec_seg<W, B>(r);
+    BoxG bx = box_a();
+    Seg l = seg_b();
     V2 d0 = l.p - bx.p;
     float lx = d0.x * bx.c + d0.y * bx.s, ly = d0.y * bx.c - d0.x * bx.s;
     float ex = l.half * fabsf(l.c * bx.c + l.s * bx.s), ey = l.half * fabsf(l.s * bx.c - l.c * bx.s);
-    if (!(fabsf(lx) - ex > bx.half_l + it.dmin_base + SPEC_FAR_MARGIN ||
-          fabsf(ly) - ey > bx.half_w + it.dmin_base + SPEC_FAR_MARGIN)) {
+    if (!(fabsf(lx) - ex > sel(LIM_L0, LIM_L1) || fabsf(ly) - ey > sel(LIM_W0, LIM_W1))) {
       Pair c = closest_box_seg(bx, l);
       V2 inner = c.a;
       float d = 0.f;
       if constexpr (!(ea.flags & VMAS_F_HOLLOW)) inner = inner_point_box(c.b, c.a, bx.p, &d);
-      f = constraint_force(inner, c.b, it.dmin_base + d, cfg.collision_force, cfg.contact_margin, false);
+      f = constraint_force(inner, c.b, dmin + d, cfg.collision_force, cfg.contact_margin, false);
       ta = cross2(c.a - bx.p, f);
       tb = cross2(c.b - l.p, neg(f));
     }
   } else if constexpr (it.kind == VMAS_K_BB) {
-    BoxG b1 = spec_box<W, A>(r), b2 = spec_box<W, B>(r);
-    if (!spec_far_apart(b1.p, b2.p, ea.circ_r + eb.circ_r + it.dmin_base)) {
+    BoxG b1 = box_a(), b2 = box_b();
+    const float circ = sel(W::ent[A0].circ_r + W::ent[B0].circ_r, W::ent[A1].circ_r + W::ent[B1].circ_r);
+    if (!spec_far_apart(b1.p, b2.p, circ + dmin)) {
       Pair c = closest_box_box(b1, b2);
       V2 in1 = c.a, in2 = c.b;
       float d1 = 0.f, d2 = 0.f;
       if constexpr (!(ea.flags & VMAS_F_HOLLOW)) in1 = inner_point_box(c.b, c.a, b1.p, &d1);
       if constexpr (!(eb.flags & VMAS_F_HOLLOW)) in2 = inner_point_box(c.a, c.b, b2.p, &d2);
-      f = constraint_force(in1, in2, (d1 + d2) + it.dmin_base, cfg.collision_force, cfg.contact_margin, false);
+      f = constraint_force(in1, in2, (d1 + d2) + dmin, cfg.collision_force, cfg.contact_margin, false);
       ta = cross2(c.a - b1.p, f);
       tb = cross2(c.b - b2.p, neg(f));
     }
   }
+  return ItemOut{f, ta, tb};
+}
 
-  if constexpr (TRACK && it.kind != VMAS_K_JOINT) {
-    if (f.x != 0.f || f.y != 0.f) sig |= 1u << (I & 31);  // this env took the contact branch of item I
-  }
+// false: the broad phase found item I's pair out of range in every env, the item is skipped
+template <class W, int I>
+DEVI bool spec_item_on(const SpecArgs& a, const uint32_t* mask_words) {
+  constexpr int bit = W::item[I].mask_bit;
+  if constexpr (bit >= 0) return !a.use_mask || ((mask_words[bit >> 5] >> (bit & 31)) & 1u);
+  return true;
+}
+
+// item I's contribution into the env's force registers, in the reference's order
+template <class W, int I, int E>
+DEVI void spec_item_add(EnvRegs<E>& r, const ItemOut& o) {
+  constexpr ItemC it = W::item[I];
+  constexpr int A = it.a, B = it.b;
+  constexpr EntC ea = W::ent[A], eb = W::ent[B];
   if constexpr (ea.flags & VMAS_F_MOVABLE) {
-    r.Fx[A] = r.Fx[A] + f.x;
-    r.Fy[A] = r.Fy[A] + f.y;
+    r.Fx[A] = r.Fx[A] + o.f.x;
+    r.Fy[A] = r.Fy[A] + o.f.y;
   }
-  if constexpr (ea.flags & VMAS_F_ROTATABLE) r.T[A] = r.T[A] + ta;
+  if constexpr (ea.flags & VMAS_F_ROTATABLE) r.T[A] = r.T[A] + o.ta;
   if constexpr (eb.flags & VMAS_F_MOVABLE) {
-    r.Fx[B] = r.Fx[B] + (-f.x);
-    r.Fy[B] = r.Fy[B] + (-f.y);
+    r.Fx[B] = r.Fx[B] + (-o.f.x);
+    r.Fy[B] = r.Fy[B] + (-o.f.y);
   }
-  if constexpr (eb.flags & VMAS_F_ROTATABLE) r.T[B] = r.T[B] + tb;
+  if constexpr (eb.flags & VMAS_F_ROTATABLE) r.T[B] = r.T[B] + o.tb;
+}
+
+// One work item evaluated and accumulated by the thread that owns the env.
+// TRACK: also record in `sig` whether the item produced a force (env scheduling; off in the default kernel)
+template <class W, int I, bool TRACK, int E>
+DEVI void spec_item(EnvRegs<E>& r, const SpecArgs& a, long env, const uint32_t* mask_words, uint32_t& sig) {
+  if (!spec_item_on<W, I>(a, mask_words)) return;
+  const ItemOut o = spec_item_eval<W, I, I>(r, a, env, false);
+  if constexpr (TRACK && W::item[I].kind != VMAS_K_JOINT) {
+    if (o.f.x != 0.f || o.f.y != 0.f) sig |= 1u << (I & 31);  // this env took the contact branch of item I
+  }
+  spec_item_add<W, I>(r, o);
+}
+
+// ---------------------------------------------------------------------------------------------
+// The lane-pair step (step_env_kernel with G = 2): the two lanes 2k, 2k+1 of a warp own one env, both hold its
+// whole state.  The work items go in rounds of up to G consecutive items that run the same code; in a round
+// each lane evaluates one item, the pair swaps the results with a shuffle and both add every item of the round
+// in item order.  Every item reads the state of the substep's start, so the sums are the thread-per-env sums,
+// bit for bit.  G = 1: a round is one item, nothing is exchanged: the thread-per-env step.
+// ---------------------------------------------------------------------------------------------
+template <class W, int G>
+struct SpecRounds {
+  static_assert(G == 1 || G == 2, "one or two lanes per env");
+  struct Table {
+    int n;
+    int first[W::NI + 1];  // round k: items first[k] .. first[k + 1] - 1
+  };
+  static constexpr Table make() {
+    Table t{};
+    int i = 0;
+    while (i < W::NI) {
+      t.first[t.n++] = i;
+      int j = i + 1;
+      while (j < W::NI && j - i < G && spec_same_code<W>(i, j)) ++j;
+      i = j;
+    }
+    t.first[t.n] = W::NI;
+    return t;
+  }
+  static constexpr Table table = make();
+  static constexpr int N = table.n;
+  // the items of round K on the even / odd lane (the same item if the round has only one)
+  template <int K>
+  static constexpr int I0 = table.first[K];
+  template <int K>
+  static constexpr int I1 = table.first[K + 1] - 1;
+};
+
+// this lane's item of round K (zero if the broad phase skips it)
+template <class W, int G, int K, int E>
+DEVI ItemOut spec_round_eval(const EnvRegs<E>& r, const SpecArgs& a, long env, const uint32_t* mask_words, bool odd) {
+  constexpr int I0 = SpecRounds<W, G>::template I0<K>, I1 = SpecRounds<W, G>::template I1<K>;
+  ItemOut o{mk(0.f, 0.f), 0.f, 0.f};
+  if (odd ? spec_item_on<W, I1>(a, mask_words) : spec_item_on<W, I0>(a, mask_words))
+    o = spec_item_eval<W, I0, I1>(r, a, env, odd);
+  return o;
+}
+
+// every item of round K into the force registers, in item order: `own` from this lane's spec_round_eval,
+// `other` from its partner's
+template <class W, int G, int K, int E>
+DEVI void spec_round_add(EnvRegs<E>& r, const SpecArgs& a, const uint32_t* mask_words, const ItemOut& own,
+                         const ItemOut& other, bool odd) {
+  constexpr int I0 = SpecRounds<W, G>::template I0<K>, I1 = SpecRounds<W, G>::template I1<K>;
+  if (spec_item_on<W, I0>(a, mask_words)) spec_item_add<W, I0>(r, I0 == I1 || !odd ? own : other);
+  if constexpr (I1 != I0) {
+    if (spec_item_on<W, I1>(a, mask_words)) spec_item_add<W, I1>(r, odd ? own : other);
+  }
+}
+
+// the sin / cos evaluations of a substep in spec_trig's order: evaluation k is of entity spec_trig_call(k) / 2,
+// of its rotation + pi / 2 if the call is odd (the second axis of a box)
+template <class W>
+__host__ __device__ constexpr int spec_trig_call(int k) {
+  for (int e = 0; e < W::E; ++e) {
+    if (!(W::ent[e].flags & VMAS_F_TRIG)) continue;
+    if (k-- == 0) return 2 * e;
+    if (W::ent[e].shape == VMAS_SHAPE_BOX && k-- == 0) return 2 * e + 1;
+  }
+  return -1;
+}
+template <class W>
+__host__ __device__ constexpr int spec_n_trig() {
+  int n = 0;
+  while (spec_trig_call<W>(n) >= 0) ++n;
+  return n;
+}
+
+// evaluations 2K, 2K + 1 spread over a lane pair (G = 1: evaluation K): this lane's sin / cos
+template <class W, int G, int K, int E>
+DEVI void spec_trig_round_eval(const EnvRegs<E>& r, bool odd, float& s, float& c) {
+  constexpr int C0 = spec_trig_call<W>(G * K), C1 = spec_trig_call<W>(G * K + G - 1 < spec_n_trig<W>() ? G * K + G - 1 : G * K);
+  const float x0 = (C0 & 1) ? r.rot[C0 / 2] + SPEC_HALF_PI_F : r.rot[C0 / 2];
+  const float x1 = (C1 & 1) ? r.rot[C1 / 2] + SPEC_HALF_PI_F : r.rot[C1 / 2];
+  sincosf(C0 != C1 && odd ? x1 : x0, &s, &c);
+}
+template <class W, int G, int K, int E>
+DEVI void spec_trig_round_put(EnvRegs<E>& r, bool odd, float s, float c, float s_other, float c_other) {
+  constexpr int C0 = spec_trig_call<W>(G * K), C1 = spec_trig_call<W>(G * K + G - 1 < spec_n_trig<W>() ? G * K + G - 1 : G * K);
+  auto put = [&](auto ci, float sv, float cv) {
+    constexpr int C = decltype(ci)::value;
+    if constexpr (C & 1) {
+      r.s2[C / 2] = sv;
+      r.c2[C / 2] = cv;
+    } else {
+      r.s[C / 2] = sv;
+      r.c[C / 2] = cv;
+    }
+  };
+  if constexpr (C0 == C1) {
+    put(std::integral_constant<int, C0>{}, s, c);
+  } else {
+    put(std::integral_constant<int, C0>{}, odd ? s_other : s, odd ? c_other : c);
+    put(std::integral_constant<int, C1>{}, odd ? s : s_other, odd ? c : c_other);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -509,10 +696,11 @@ struct SpecRows {
       }
     });
   }
-  // registers -> rows -> global: vector stores of the chunks that hold a changed column
+  // registers -> rows -> global: vector stores of the chunks that hold a changed column.  `lanes` lanes own the
+  // env: `lane` stores the rows j = lane (mod lanes) of (pos, vel, rot, ang_vel, force, torque)
   template <int NAX>
   DEVI void store(const SpecArgs& a, const long env, const EnvRegs<E>& r, const float (&afx)[NAX],
-                  const float (&afy)[NAX], const float (&atq)[NAX]) {
+                  const float (&afy)[NAX], const float (&atq)[NAX], const int lanes = 1, const int lane = 0) {
     static_for<E>([&](auto ei) {
       constexpr int e = decltype(ei)::value;
       constexpr EntC en = W::ent[e];
@@ -535,12 +723,12 @@ struct SpecRows {
           t[en.agent] = atq[en.agent];
       }
     });
-    row_store<2 * E, VEL_IO>(a.st.pos + (size_t)env * 2 * E, pos);
-    row_store<2 * E, VEL_IO>(a.st.vel + (size_t)env * 2 * E, vel);
-    row_store<E, ROT_ST>(a.st.rot + (size_t)env * E, rot);
-    row_store<E, ROT_ST>(a.st.ang_vel + (size_t)env * E, w);
-    row_store<2 * NA, F_ST>(a.st.force + (size_t)env * 2 * NA, f);
-    row_store<NA, T_ST>(a.st.torque + (size_t)env * NA, t);
+    if (lane == 0 % lanes) row_store<2 * E, VEL_IO>(a.st.pos + (size_t)env * 2 * E, pos);
+    if (lane == 1 % lanes) row_store<2 * E, VEL_IO>(a.st.vel + (size_t)env * 2 * E, vel);
+    if (lane == 2 % lanes) row_store<E, ROT_ST>(a.st.rot + (size_t)env * E, rot);
+    if (lane == 3 % lanes) row_store<E, ROT_ST>(a.st.ang_vel + (size_t)env * E, w);
+    if (lane == 4 % lanes) row_store<2 * NA, F_ST>(a.st.force + (size_t)env * 2 * NA, f);
+    if (lane == 5 % lanes) row_store<NA, T_ST>(a.st.torque + (size_t)env * NA, t);
   }
 };
 
@@ -611,8 +799,23 @@ DEVI void spec_epilogue_prefetch(const EpiArgs& e, const long env) {
 #endif
 }
 
-template <class W, class P>
-DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs& e, const long env) {
+// `lanes` lanes own the env (each holds its whole state and runs the program): `lane` writes the shaping carry
+// if it is lane 0, the program's STOREs j = lane (mod lanes) and the observation rows r = lane (mod lanes)
+template <class P>
+__host__ __device__ constexpr int epi_store_index(int i) {
+  int n = 0;
+  for (int j = 0; j < i; ++j) n += P::prog[j].op == VMAS_OP_STORE_F32 || P::prog[j].op == VMAS_OP_STORE_BOOL;
+  return n;
+}
+
+struct EpiOneLane {
+  DEVI float operator()(float v) const { return v; }
+};
+
+// from_lane0(v): the value v of lane 0 of the env's lanes (the shaping carry, read by lane 0 only: it overwrites it)
+template <class W, class P, class X = EpiOneLane>
+DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs& e, const long env,
+                        const int lanes = 1, const int lane = 0, X from_lane0 = {}) {
   // the step program (ref scenarios/balance.py:197-263 as a StepProgram; see vmas_b200_post_step)
   float pr[VMAS_PROG_REGS];
 #pragma unroll
@@ -630,9 +833,11 @@ DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs
       const float d = norm2(r.px[ia] - r.px[ib], r.py[ia] - r.py[ib]);
       const float shaping = d * in.imm;
       float* prev = static_cast<float*>(e.buffers[in.a]) + env;
-      pr[in.dst] = *prev - shaping;
+      float carry = 0.f;
+      if (lane == 0) carry = *prev;
+      pr[in.dst] = from_lane0(carry) - shaping;
       pr[in.dst + 1] = d;
-      *prev = shaping;
+      if (lane == 0) *prev = shaping;
     } else if constexpr (in.op == VMAS_OP_LOAD_F32) {
       pr[in.dst] = static_cast<const float*>(e.buffers[in.a])[env];
     } else if constexpr (in.op == VMAS_OP_LOAD_BOOL) {
@@ -664,9 +869,10 @@ DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs
     } else if constexpr (in.op == VMAS_OP_WHERE) {
       pr[in.dst] = pr[in.a] != 0.f ? pr[in.b] : pr[in.arg & 0xFF];
     } else if constexpr (in.op == VMAS_OP_STORE_F32) {
-      static_cast<float*>(e.buffers[in.b])[env] = pr[in.a];
+      if (lane == epi_store_index<P>(decltype(ii)::value) % lanes) static_cast<float*>(e.buffers[in.b])[env] = pr[in.a];
     } else if constexpr (in.op == VMAS_OP_STORE_BOOL) {
-      static_cast<uint8_t*>(e.buffers[in.b])[env] = pr[in.a] != 0.f ? 1 : 0;
+      if (lane == epi_store_index<P>(decltype(ii)::value) % lanes)
+        static_cast<uint8_t*>(e.buffers[in.b])[env] = pr[in.a] != 0.f ? 1 : 0;
     }
   });
   // the observation rows (ref scenarios/balance.py:236-262 as an ObservationPlan): [rows, B, width]
@@ -675,6 +881,7 @@ DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs
     constexpr int VEC = F % 4 == 0 ? 4 : 1;
     static_for<P::OBS_ROWS>([&](auto ri) {
       constexpr int row = decltype(ri)::value;
+      if (lane != row % lanes) return;
       float* dst = e.obs_out + ((size_t)row * a.batch_dim + env) * F;
       static_for<F / VEC>([&](auto gi) {
         constexpr int c0 = decltype(gi)::value * VEC;
@@ -831,10 +1038,54 @@ DEVI unsigned ld_acquire_u32(const uint32_t* p) {
   return v;
 }
 
-template <class W, class P>
-__global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_env_kernel(const SpecArgs a, const EpiArgs e, const ActArgs act) {
-  constexpr int MW = W::MASK_WORDS, E = W::E, NA = W::A, NI = W::NI;
-  const long tid = (long)blockIdx.x * W::BLOCK + threadIdx.x;
+// the k-th masked work item, in item order
+template <class W>
+__host__ __device__ constexpr int spec_masked_item(int k) {
+  for (int i = 0; i < W::NI; ++i)
+    if (W::item[i].mask_bit >= 0 && k-- == 0) return i;
+  return -1;
+}
+template <class W>
+__host__ __device__ constexpr int spec_n_masked() {
+  int n = 0;
+  for (int i = 0; i < W::NI; ++i) n += W::item[i].mask_bit >= 0;
+  return n;
+}
+
+// the partner lane's value (lanes 2k, 2k + 1)
+DEVI float pair_swap(float v) { return __shfl_xor_sync(0xffffffffu, v, 1); }
+
+// what the partner lane evaluated in round K (only the parts some item of the round adds somewhere)
+template <class W, int G, int K>
+DEVI ItemOut spec_round_swap(const ItemOut& o) {
+  constexpr int I0 = SpecRounds<W, G>::template I0<K>, I1 = SpecRounds<W, G>::template I1<K>;
+  if constexpr (I0 == I1) {
+    return o;
+  } else {
+    constexpr int fa = W::ent[W::item[I0].a].flags | W::ent[W::item[I1].a].flags;
+    constexpr int fb = W::ent[W::item[I0].b].flags | W::ent[W::item[I1].b].flags;
+    ItemOut p = o;
+    if constexpr ((fa | fb) & VMAS_F_MOVABLE) {
+      p.f.x = pair_swap(o.f.x);
+      p.f.y = pair_swap(o.f.y);
+    }
+    if constexpr (fa & VMAS_F_ROTATABLE) p.ta = pair_swap(o.ta);
+    if constexpr (fb & VMAS_F_ROTATABLE) p.tb = pair_swap(o.tb);
+    return p;
+  }
+}
+
+// G lanes per env (see SpecRounds): lanes 2k, 2k + 1 of a warp own one env, a block holds W::BLOCK envs whatever
+// G.  Both lanes load the env's rows (the same addresses: no extra bytes) and keep its whole state; they split
+// the action ingest, the broad-phase tests, the sin / cos evaluations, the work items, the row stores, the
+// program's stores and the observation rows, and exchange what the other lane needs by shuffles.
+template <class W, class P, int G>
+__global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_BLOCKS / G : 1))
+    step_env_kernel(const SpecArgs a, const EpiArgs e, const ActArgs act) {
+  constexpr int MW = W::MASK_WORDS, E = W::E, NA = W::A;
+  using R = SpecRounds<W, G>;
+  const long tid = ((long)blockIdx.x * (W::BLOCK * G) + threadIdx.x) / G;
+  const bool odd = G > 1 && (threadIdx.x & 1);
   const bool live = tid < a.batch_dim;
   const long env = live ? tid : (long)a.batch_dim - 1;  // (the tail threads shadow the last env and store nothing)
   SpecRows<W, true> rows;
@@ -848,23 +1099,34 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_env_kernel(const
   float afx[NA > 0 ? NA : 1], afy[NA > 0 ? NA : 1], atq[NA > 0 ? NA : 1];
   rows.unpack_pos_rot(r);
   rows.unpack_rest(r, afx, afy, atq);
-  // the actions
+  // the actions: agents k0 = G j and k1 = G j + G - 1 on the lanes of a pair
   bool bad = false;
-  static_for<P::N_ACT>([&](auto ki) {
-    constexpr int k = decltype(ki)::value;
-    constexpr ActC ac = P::act[k];
-    float2 v = reinterpret_cast<const float2*>(act.actions[k])[env];
+  static_for<(P::N_ACT + G - 1) / G>([&](auto ji) {
+    constexpr int k0 = decltype(ji)::value * G, k1 = k0 + G - 1 < P::N_ACT ? k0 + G - 1 : k0;
+    constexpr ActC c0 = P::act[k0], c1 = P::act[k1];
+    const bool o = k0 != k1 && odd;
+    const float range0 = o ? c1.range0 : c0.range0, range1 = o ? c1.range1 : c0.range1;
+    float2 v = reinterpret_cast<const float2*>(o ? act.actions[k1] : act.actions[k0])[env];
     if (act.clamp) {  // torch.clamp keeps NaN
-      v.x = fminf(fmaxf(v.x, -ac.range0), ac.range0);
-      v.y = fminf(fmaxf(v.y, -ac.range1), ac.range1);
+      v.x = fminf(fmaxf(v.x, -range0), range0);
+      v.y = fminf(fmaxf(v.y, -range1), range1);
     }
-    bad |= (v.x != v.x) || (fabsf(v.x) > ac.range0) || (v.y != v.y) || (fabsf(v.y) > ac.range1);
-    const float2 u = make_float2(v.x * ac.mult0, v.y * ac.mult1);
-    if (live) reinterpret_cast<float2*>(act.u[k])[env] = u;
-    afx[ac.agent] = u.x;
-    afy[ac.agent] = u.y;
+    bad |= (v.x != v.x) || (fabsf(v.x) > range0) || (v.y != v.y) || (fabsf(v.y) > range1);
+    const float2 u = make_float2(v.x * (o ? c1.mult0 : c0.mult0), v.y * (o ? c1.mult1 : c0.mult1));
+    if (live && (k0 != k1 || !odd)) reinterpret_cast<float2*>(o ? act.u[k1] : act.u[k0])[env] = u;
+    if constexpr (k0 == k1) {
+      afx[c0.agent] = u.x;
+      afy[c0.agent] = u.y;
+    } else {
+      const float2 p = make_float2(pair_swap(u.x), pair_swap(u.y));
+      afx[c0.agent] = odd ? p.x : u.x;
+      afy[c0.agent] = odd ? p.y : u.y;
+      afx[c1.agent] = odd ? u.x : p.x;
+      afy[c1.agent] = odd ? u.y : p.y;
+    }
   });
-  if (live) {
+  if constexpr (G > 1) bad = __shfl_xor_sync(0xffffffffu, (int)bad, 1) || bad;
+  if (live && !odd) {
     if (bad && act.bad_flag) *act.bad_flag = 1;
     if (act.steps) act.steps[env] = act.steps[env] + 1.f;
   }
@@ -887,11 +1149,20 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_env_kernel(const
         uint32_t bits[MW];
 #pragma unroll
         for (int w = 0; w < MW; ++w) bits[w] = 0u;
-        static_for<NI>([&](auto ii) {
-          constexpr ItemC it = W::item[decltype(ii)::value];
-          if constexpr (it.mask_bit >= 0) {
-            const bool near = live && norm2(r.px[it.a] - r.px[it.b], r.py[it.a] - r.py[it.b]) <= it.broad_thr;
-            if (__any_sync(0xffffffffu, near)) bits[it.mask_bit >> 5] |= 1u << (it.mask_bit & 31);
+        // masked items m0, m1 on the even / odd lanes; a warp's even lanes vote for m0, its odd lanes for m1
+        static_for<(spec_n_masked<W>() + G - 1) / G>([&](auto ji) {
+          constexpr int j0 = decltype(ji)::value * G, j1 = j0 + G - 1 < spec_n_masked<W>() ? j0 + G - 1 : j0;
+          constexpr ItemC i0 = W::item[spec_masked_item<W>(j0)], i1 = W::item[spec_masked_item<W>(j1)];
+          const bool o = j0 != j1 && odd;
+          const bool near = live && norm2((o ? r.px[i1.a] : r.px[i0.a]) - (o ? r.px[i1.b] : r.px[i0.b]),
+                                          (o ? r.py[i1.a] : r.py[i0.a]) - (o ? r.py[i1.b] : r.py[i0.b])) <=
+                                        (o ? i1.broad_thr : i0.broad_thr);
+          if constexpr (j0 == j1) {
+            if (__any_sync(0xffffffffu, near)) bits[i0.mask_bit >> 5] |= 1u << (i0.mask_bit & 31);
+          } else {
+            const unsigned vote = __ballot_sync(0xffffffffu, near);
+            if (vote & 0x55555555u) bits[i0.mask_bit >> 5] |= 1u << (i0.mask_bit & 31);
+            if (vote & 0xAAAAAAAAu) bits[i1.mask_bit >> 5] |= 1u << (i1.mask_bit & 31);
           }
         });
         if ((threadIdx.x & 31) == 0) {
@@ -910,11 +1181,19 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_env_kernel(const
         }
       }
     }
-    spec_trig<W>(r);
+    static_for<(spec_n_trig<W>() + G - 1) / G>([&](auto ki) {
+      constexpr int K = decltype(ki)::value;
+      float s, c;
+      spec_trig_round_eval<W, G, K>(r, odd, s, c);
+      if constexpr (G * K + 1 < spec_n_trig<W>() && G > 1)
+        spec_trig_round_put<W, G, K>(r, odd, s, c, pair_swap(s), pair_swap(c));
+      else
+        spec_trig_round_put<W, G, K>(r, odd, s, c, s, c);
+    });
     spec_entity_forces<W>(r, afx, afy, atq);
-    static_for<NI>([&](auto ii) {
-      constexpr int I = decltype(ii)::value;
-      if constexpr (MW > 0 && I == spec_first_masked<W>()) {
+    static_for<R::N>([&](auto ki) {
+      constexpr int K = decltype(ki)::value;
+      if constexpr (MW > 0 && R::template I0<K> == spec_first_masked<W>()) {
         if (a.use_mask) {  // WAIT
           if (threadIdx.x == 0) {
             while (ld_acquire_u32(&gmask[MW]) < gridDim.x) __nanosleep(20);
@@ -930,41 +1209,73 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_env_kernel(const
           for (int w = 0; w < MW; ++w) mask_words[w] = s_mask[w];
         }
       }
-      spec_item<W, I, false>(r, a, env, mask_words, sig);
+      if constexpr (R::template I0<K> == R::template I1<K>) {  // a lone item: both lanes evaluate it
+        spec_item<W, R::template I0<K>, false>(r, a, env, mask_words, sig);
+      } else {
+        const ItemOut own = spec_round_eval<W, G, K>(r, a, env, mask_words, odd);
+        spec_round_add<W, G, K>(r, a, mask_words, own, spec_round_swap<W, G, K>(own), odd);
+      }
     });
     spec_integrate<W>(r, sub);
   }
   if (!live) return;
-  rows.store(a, env, r, afx, afy, atq);
-  spec_epilogue<W, P>(r, a, e, env);
+  rows.store(a, env, r, afx, afy, atq, G, odd ? 1 : 0);
+  spec_epilogue<W, P>(r, a, e, env, G, odd ? 1 : 0, [odd](float v) {
+    if constexpr (G == 1) return v;
+    const float v0 = __shfl_xor_sync(0x3u << (threadIdx.x & 30), v, 1);  // (both lanes of a pair are here)
+    return odd ? v0 : v;
+  });
 }
 
-// cudaErrorCooperativeLaunchTooLarge: the batch does not fit the GPU at once (masked worlds only)
+// resident blocks of step_env_kernel<W, P, G> on the current device (occupancy query, once per device)
+template <class W, class P, int G>
+static cudaError_t env_capacity(long& cap) {
+  static long capacity[64] = {0};
+  int device = 0;
+  cudaError_t err = cudaGetDevice(&device);
+  if (err != cudaSuccess) return err;
+  cap = device < 64 ? capacity[device] : 0;
+  if (cap == 0) {
+    int per_sm = 0, sms = 0;
+    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_env_kernel<W, P, G>, W::BLOCK * G, 0);
+    if (err != cudaSuccess) return err;
+    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err != cudaSuccess) return err;
+    cap = (long)per_sm * sms;
+    if (device < 64) capacity[device] = cap;
+  }
+  return cudaSuccess;
+}
+
+template <class W, class P, int G>
+static cudaError_t launch_env_lanes(const SpecArgs& a, const EpiArgs& e, const ActArgs& act, long blocks, bool coop,
+                                    cudaStream_t stream) {
+  if (coop) {
+    void* args[] = {const_cast<SpecArgs*>(&a), const_cast<EpiArgs*>(&e), const_cast<ActArgs*>(&act)};
+    return cudaLaunchCooperativeKernel(reinterpret_cast<void*>(step_env_kernel<W, P, G>), dim3((unsigned)blocks),
+                                       dim3(W::BLOCK * G), args, 0, stream);
+  }
+  step_env_kernel<W, P, G><<<(unsigned)blocks, W::BLOCK * G, 0, stream>>>(a, e, act);
+  return cudaGetLastError();
+}
+
+// Two lanes per env while every block fits the GPU at once, else one: that holds twice the envs resident, which
+// the grid barrier of a masked world needs.  cudaErrorCooperativeLaunchTooLarge: the batch does not fit the GPU
+// at once even so (masked worlds only)
 template <class W, class P>
 static cudaError_t launch_env(const SpecArgs& a, const EpiArgs& e, const ActArgs& act, cudaStream_t stream) {
   const long blocks = ((long)a.batch_dim + W::BLOCK - 1) / W::BLOCK;
-  if (W::MASK_WORDS > 0 && a.use_mask) {
-    static long capacity[64] = {0};
-    int device = 0;
-    cudaError_t err = cudaGetDevice(&device);
+  const bool coop = W::MASK_WORDS > 0 && a.use_mask;
+  long cap = 0;
+  cudaError_t err = env_capacity<W, P, 2>(cap);
+  if (err != cudaSuccess) return err;
+  if (blocks <= cap) return launch_env_lanes<W, P, 2>(a, e, act, blocks, coop, stream);
+  if (coop) {
+    err = env_capacity<W, P, 1>(cap);
     if (err != cudaSuccess) return err;
-    long cap = device < 64 ? capacity[device] : 0;
-    if (cap == 0) {
-      int per_sm = 0, sms = 0;
-      err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_env_kernel<W, P>, W::BLOCK, 0);
-      if (err != cudaSuccess) return err;
-      err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-      if (err != cudaSuccess) return err;
-      cap = (long)per_sm * sms;
-      if (device < 64) capacity[device] = cap;
-    }
     if (blocks > cap) return cudaErrorCooperativeLaunchTooLarge;
-    void* args[] = {const_cast<SpecArgs*>(&a), const_cast<EpiArgs*>(&e), const_cast<ActArgs*>(&act)};
-    return cudaLaunchCooperativeKernel(reinterpret_cast<void*>(step_env_kernel<W, P>), dim3((unsigned)blocks),
-                                       dim3(W::BLOCK), args, 0, stream);
   }
-  step_env_kernel<W, P><<<(unsigned)blocks, W::BLOCK, 0, stream>>>(a, e, act);
-  return cudaGetLastError();
+  return launch_env_lanes<W, P, 1>(a, e, act, blocks, coop, stream);
 }
 
 template <class W, class P>
