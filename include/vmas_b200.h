@@ -36,15 +36,21 @@ enum {
   VMAS_F_MOVABLE = 1 << 0, VMAS_F_ROTATABLE = 1 << 1, VMAS_F_HOLLOW = 1 << 2, VMAS_F_AGENT = 1 << 3,
   VMAS_F_LIN_FRIC = 1 << 4, VMAS_F_ANG_FRIC = 1 << 5, VMAS_F_GRAVITY = 1 << 6, VMAS_F_MAX_SPEED = 1 << 7,
   VMAS_F_V_RANGE = 1 << 8, VMAS_F_MAX_F = 1 << 9, VMAS_F_F_RANGE = 1 << 10, VMAS_F_MAX_T = 1 << 11,
-  VMAS_F_T_RANGE = 1 << 12, VMAS_F_TRIG = 1 << 13, VMAS_F_GRAVITY_ENV = 1 << 14
+  VMAS_F_T_RANGE = 1 << 12, VMAS_F_TRIG = 1 << 13, VMAS_F_GRAVITY_ENV = 1 << 14,
+  /* per-env mass / friction coefficients, read from the ent_params table of vmas_b200_world_step_params */
+  VMAS_F_MASS_ENV = 1 << 15, VMAS_F_LIN_FRIC_ENV = 1 << 16, VMAS_F_ANG_FRIC_ENV = 1 << 17
 };
 /* columns of ent_f32 [E, 20] */
 enum {
   VMAS_EF_D0 = 0, VMAS_EF_D1, VMAS_EF_MASS, VMAS_EF_INERTIA, VMAS_EF_DRAG_MULT, VMAS_EF_LIN_FRIC,
   VMAS_EF_ANG_FRIC, VMAS_EF_GRAV_X, VMAS_EF_GRAV_Y, VMAS_EF_MAX_SPEED, VMAS_EF_V_RANGE, VMAS_EF_MAX_F,
   VMAS_EF_F_RANGE, VMAS_EF_MAX_T, VMAS_EF_T_RANGE, VMAS_EF_CIRC_R, VMAS_EF_R_PLUS_LMD,
+  /* VMAS_F_MASS_ENV: moment of inertia = fp32(fp32(K0 * mass) * K1) (ref core.py:123-124, 160-161, 187-188) */
+  VMAS_EF_INERTIA_K0, VMAS_EF_INERTIA_K1,
   VMAS_EF_COLS = 20
 };
+/* columns of the per-env parameter table ent_params [B, E, VMAS_EP_COLS] */
+enum { VMAS_EP_MASS = 0, VMAS_EP_LIN_FRIC = 1, VMAS_EP_ANG_FRIC = 2, VMAS_EP_COLS = 4 };
 /* columns of item_f32 [NI, 8] */
 enum {
   VMAS_IF_BROAD_THR = 0, VMAS_IF_DMIN_BASE, VMAS_IF_AX, VMAS_IF_AY, VMAS_IF_BX, VMAS_IF_BY, VMAS_IF_DIST,
@@ -147,6 +153,20 @@ int vmas_b200_specialization_has_tile(int index);
  */
 int vmas_b200_world_step(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,
                          uint32_t* mask, int exact_broad_phase, void* cuda_stream);
+
+/*
+ * vmas_b200_world_step for a world whose entities carry per-env physical parameters (domain
+ * randomisation: ref core.py:2043-2102, 2870 with a [B, 1] Entity.mass / friction coefficient).
+ *   ent_params  device fp32 [B, E, VMAS_EP_COLS]: mass, linear-friction coefficient, angular-friction
+ *               coefficient, unused.  Only the columns an entity's VMAS_F_*_ENV flags name are read, and only
+ *               for flagged entities; the rest of the table is never touched.  NULL: no entity is flagged
+ *               (vmas_b200_world_step is this call with NULL).  A specialised world with flagged entities
+ *               called with NULL fails with an error; the generic kernels then read the description's
+ *               placeholder scalars, never the table.
+ * Per-env gravity (VMAS_F_GRAVITY_ENV) is read from VmasPlanTables.ent_gravity as before.
+ */
+int vmas_b200_world_step_params(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const float* ent_params,
+                                const VmasState* st, uint32_t* mask, int exact_broad_phase, void* cuda_stream);
 
 /*
  * Same as vmas_b200_world_step, additionally recording two caller-owned CUDA events

@@ -238,6 +238,7 @@ EXPORTS = [
     "vmas_b200_specialization_has_tile",
     "vmas_b200_register_specialization",
     "vmas_b200_world_step",
+    "vmas_b200_world_step_params",
     "vmas_b200_world_substeps",
     "vmas_b200_world_step_timed",
     "vmas_b200_cast_rays",
@@ -284,6 +285,7 @@ def load():
     lib.vmas_b200_last_error.restype = C.c_char_p
     p_cfg, p_tb, p_st = C.POINTER(WorldConfig), C.POINTER(PlanTablesC), C.POINTER(StateC)
     lib.vmas_b200_world_step.argtypes = [p_cfg, p_tb, p_st, C.c_void_p, C.c_int, C.c_void_p]
+    lib.vmas_b200_world_step_params.argtypes = [p_cfg, p_tb, C.c_void_p, p_st, C.c_void_p, C.c_int, C.c_void_p]
     lib.vmas_b200_world_substeps.argtypes = [
         p_cfg, p_tb, p_st, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p
     ]
@@ -490,6 +492,17 @@ class DeviceTables:
             if self.gravity_entities
             else None
         )
+        # per-env mass / friction coefficients: [B, E, EP_COLS], the rows of flagged entities written before each
+        # step (CudaBackend._sync_entity_params)
+        self.param_entities = [
+            i for i, e in enumerate(desc.entities)
+            if e.get("mass_per_env") or e.get("lin_fric_per_env") or e.get("ang_fric_per_env")
+        ]
+        self.ent_params = (
+            torch.zeros(B, desc.n_entities, P.EP_COLS, dtype=torch.float32, device=self.device)
+            if self.param_entities
+            else None
+        )
         words = (tables.n_masked + 31) // 32
         # (+ the kernels' arrival counters; the one-kernel step keeps a mask per substep)
         self.mask = torch.zeros(max(1, int(tables.desc.substeps)) * (words + 2), dtype=torch.int32, device=self.device)
@@ -547,7 +560,16 @@ def world_step(lib, dt: DeviceTables, slab, exact_broad_phase: bool = True, even
     """One World.step.  ``events``: optional (begin, end) torch.cuda.Event pair (timing enabled)
     recorded around the substep kernel(s) only."""
     st = dt.state_struct(slab)
-    if events is None:
+    if dt.ent_params is not None:
+        if events is not None:
+            events[0].record()
+        rc = lib.vmas_b200_world_step_params(
+            C.byref(dt.cfg), C.byref(dt.tb), dt.ent_params.data_ptr(), C.byref(st), dt.mask.data_ptr(),
+            int(exact_broad_phase), _stream(dt.device),
+        )
+        if events is not None:
+            events[1].record()
+    elif events is None:
         rc = lib.vmas_b200_world_step(
             C.byref(dt.cfg), C.byref(dt.tb), C.byref(st), dt.mask.data_ptr(), int(exact_broad_phase),
             _stream(dt.device),

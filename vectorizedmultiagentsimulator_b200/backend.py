@@ -152,6 +152,9 @@ class CudaBackend(PlanRuntime):
         if job.index >= 0:
             self._dev_tables = self._native.DeviceTables(self.tables, self.world, self.device)
             self._fixed_rot_versions = {}
+            # a broad-phase mask the action ingest of this step built went to the old tables' scratch: the
+            # coming step builds its own in the new tables
+            self._mask_ready = False
         elif job.error:
             import warnings
 
@@ -189,12 +192,30 @@ class CudaBackend(PlanRuntime):
         for i in dt.gravity_entities:
             dt.ent_gravity[:, i].copy_(ents[i].gravity)
 
+    def _sync_entity_params(self):
+        """The per-env mass / friction coefficients of the flagged entities into ``ent_params`` (captured with
+        the step in graph mode: the copies read the entities' own buffers, whose addresses never change)."""
+        dt = self._dev_tables
+        if dt.ent_params is None:
+            return
+        ents, desc = self.world.entities, self.tables.desc
+        for i in dt.param_entities:
+            e, d = ents[i], desc.entities[i]
+            for flag, attr, col in (
+                ("mass_per_env", "mass", P.EP_MASS),
+                ("lin_fric_per_env", "linear_friction", P.EP_LIN_FRIC),
+                ("ang_fric_per_env", "angular_friction", P.EP_ANG_FRIC),
+            ):
+                if d[flag]:
+                    dt.ent_params[:, i, col : col + 1].copy_(getattr(e, attr))
+
     def step(self):
         self.refresh()
         if self._jit_job is not None:
             self._adopt_jit()
         self._sync_fixed_rotations()
         self._sync_entity_gravity()
+        self._sync_entity_params()
         slab = self.world.slab
         events = None
         if self.kernel_events is not None:

@@ -49,8 +49,9 @@ def world_hash(desc: P.WorldDescription) -> int:
     d.pop("batch_dim")
     for e in d["entities"]:
         e.pop("name")
-        if not e.get("gravity_per_env"):
-            e.pop("gravity_per_env", None)  # absent in descriptions written before the field existed
+        for flag in ("gravity_per_env", "mass_per_env", "lin_fric_per_env", "ang_fric_per_env"):
+            if not e.get(flag):
+                e.pop(flag, None)  # absent in descriptions written before the field existed
     blob = json.dumps(d, sort_keys=True).encode()
     h = 0xCBF29CE484222325
     for byte in blob:
@@ -63,12 +64,21 @@ def _item_cost(kind: int) -> int:
     return {P.K_JOINT: 1, P.K_SS: 1, P.K_LS: 1, P.K_LL: 1, P.K_BS: 1, P.K_BL: 4, P.K_BB: 32}[kind]
 
 
-def specializable(desc: P.WorldDescription) -> bool:
+def specializable(desc: P.WorldDescription, per_env: bool = False) -> bool:
+    """Whether ``desc`` gets the specialised kernels.  ``per_env``: worlds with per-env masses, friction
+    coefficients or gravity qualify too (their step_spec_kernel reads SpecArgs.ent_params / ent_gravity; they
+    get neither the tile kernel nor a whole-step kernel), else they do not."""
     if desc.n_entities > MAX_ENTITIES or desc.n_entities == 0:
         return False
-    if any(e.get("gravity_per_env") for e in desc.entities):
+    if not per_env and has_per_env_params(desc):
         return False
     return sum(_item_cost(it["kind"]) for it in desc.items) <= MAX_ITEM_COST
+
+
+def has_per_env_params(desc: P.WorldDescription) -> bool:
+    """Some entity's mass, friction coefficient or gravity is given per env."""
+    flags = ("gravity_per_env", "mass_per_env", "lin_fric_per_env", "ang_fric_per_env")
+    return any(e.get(f) for e in desc.entities for f in flags)
 
 
 def _f(x) -> str:
@@ -86,6 +96,10 @@ def emit_world(desc: P.WorldDescription, label: str, tuning: Dict = None) -> Tup
     min_blocks = (tuning or {}).get("min_blocks", "SPEC_MIN_BLOCKS")
     tables = P.build_tables(desc)
     h = world_hash(desc)
+    # the entities' per-env attributes (spec_kernel.cuh reads them from SpecArgs behind `if constexpr`);
+    # emitted only when there are any, so that every other world's text stays as it was
+    env_mask = [int(f) & (P.F_GRAVITY_ENV | P.F_PARAMS_ENV) for f in tables.ent_i32[: desc.n_entities, 1]]
+    per_env = any(env_mask)
     name = f"World_{h:016x}"
     E, NI = desc.n_entities, len(desc.items)
     ef, ei = tables.ent_f32, tables.ent_i32
@@ -110,10 +124,12 @@ def emit_world(desc: P.WorldDescription, label: str, tuning: Dict = None) -> Tup
             P.EF_D0, P.EF_D1, P.EF_MASS, P.EF_INERTIA, P.EF_DRAG_MULT, P.EF_LIN_FRIC, P.EF_ANG_FRIC, P.EF_GRAV_X,
             P.EF_GRAV_Y, P.EF_MAX_SPEED, P.EF_V_RANGE, P.EF_MAX_F, P.EF_F_RANGE, P.EF_MAX_T, P.EF_T_RANGE,
             P.EF_CIRC_R, P.EF_R_PLUS_LMD,
-        ]
+        ] + ([P.EF_INERTIA_K0, P.EF_INERTIA_K1] if per_env else [])
         vals = ", ".join(_f(r[c]) for c in cols)
         lines.append(f"      {{{int(ei[e, 0])}, {int(ei[e, 1])}, {int(ei[e, 2])}, {vals}}},  // {desc.entities[e]['name']}")
     lines.append("  };")
+    if per_env:
+        lines.append(f"  static constexpr int PER_ENV[{E}] = {{{', '.join(str(m) for m in env_mask)}}};")
     lines.append(f"  static constexpr ItemC item[{max(NI, 1)}] = {{")
     if NI == 0:
         lines.append("      {0, 0, 0, 0, -1, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f},")

@@ -26,6 +26,7 @@ struct EntC {
   int shape, flags, agent;
   float d0, d1, mass, inertia, drag_mult, lin_fric, ang_fric, grav_x, grav_y, max_speed, v_range, max_f, f_range,
       max_t, t_range, circ_r, r_plus_lmd;
+  float inertia_k0, inertia_k1;  // (worlds with per-env masses only: see SpecEnvParams)
 };
 struct ItemC {
   int kind, a, b, flags, mask_bit;
@@ -76,6 +77,9 @@ struct SpecArgs {
   // records which of its work items produced a force (bit I & 31) for the next re-ordering
   const int32_t* order;  // [B] permutation of the envs, or null: thread t steps env t
   uint32_t* sig;         // [B] out, or null
+  // per-env physical parameters (worlds whose W::PER_ENV flags an entity only, see SpecEnvParams)
+  const float* ent_params;   // [B, E, VMAS_EP_COLS]: mass, linear / angular friction coefficient, or null
+  const float* ent_gravity;  // [B, E, 2], or null
 };
 
 template <class F, int... I>
@@ -500,6 +504,90 @@ __host__ __device__ constexpr uint64_t agent_cols(int flag_all, int flag_any, in
   return m;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Per-env physical parameters (domain randomisation).  A world with entities whose mass, friction
+// coefficients or gravity are given per env carries `static constexpr int PER_ENV[E]`: the
+// VMAS_F_GRAVITY_ENV | VMAS_F_*_ENV bits of each entity.  Every other world has no such member, its
+// mask reads zero and not one instruction of its kernels changes.
+// ---------------------------------------------------------------------------------------------
+template <class W, class = void>
+struct SpecPerEnv {
+  static constexpr bool any = false;
+  __host__ __device__ static constexpr int at(int) { return 0; }
+};
+template <class W>
+struct SpecPerEnv<W, std::void_t<decltype(W::PER_ENV)>> {
+  static constexpr bool any = true;
+  __host__ __device__ static constexpr int at(int e) { return W::PER_ENV[e]; }
+};
+template <class W>
+__host__ __device__ constexpr bool spec_needs_params() {
+  for (int e = 0; e < W::E; ++e)
+    if (SpecPerEnv<W>::at(e) & (VMAS_F_MASS_ENV | VMAS_F_LIN_FRIC_ENV | VMAS_F_ANG_FRIC_ENV)) return true;
+  return false;
+}
+template <class W>
+__host__ __device__ constexpr bool spec_needs_gravity() {
+  for (int e = 0; e < W::E; ++e)
+    if (SpecPerEnv<W>::at(e) & VMAS_F_GRAVITY_ENV) return true;
+  return false;
+}
+
+// One env's per-env parameters, loaded once per launch into registers (only the flagged entries exist after
+// unrolling).  The moment of inertia of a per-env mass is rounded as the reference rounds
+// `shape.moment_of_inertia(mass)` on a [B, 1] tensor: fp32(fp32(K0 * m) * K1).
+template <class W>
+struct SpecEnvParams {
+  static constexpr int E = W::E;
+  float mass[E], inertia[E], lin_fric[E], ang_fric[E], gx[E], gy[E];
+
+  DEVI void load(const SpecArgs& a, const long env) {
+    static_for<E>([&](auto ei) {
+      constexpr int e = decltype(ei)::value;
+      constexpr int m = SpecPerEnv<W>::at(e);
+      if constexpr (m & (VMAS_F_MASS_ENV | VMAS_F_LIN_FRIC_ENV | VMAS_F_ANG_FRIC_ENV)) {
+        const float4 p = reinterpret_cast<const float4*>(a.ent_params)[(size_t)env * E + e];
+        if constexpr (m & VMAS_F_MASS_ENV) {
+          mass[e] = p.x;
+          inertia[e] = (W::ent[e].inertia_k0 * p.x) * W::ent[e].inertia_k1;
+        }
+        if constexpr (m & VMAS_F_LIN_FRIC_ENV) lin_fric[e] = p.y;
+        if constexpr (m & VMAS_F_ANG_FRIC_ENV) ang_fric[e] = p.z;
+      }
+      if constexpr (m & VMAS_F_GRAVITY_ENV) {
+        const float2 g = reinterpret_cast<const float2*>(a.ent_gravity)[(size_t)env * E + e];
+        gx[e] = g.x;
+        gy[e] = g.y;
+      }
+    });
+  }
+};
+static_assert(VMAS_EP_MASS == 0 && VMAS_EP_LIN_FRIC == 1 && VMAS_EP_ANG_FRIC == 2 && VMAS_EP_COLS == 4,
+              "SpecEnvParams::load reads an ent_params row as one float4");
+
+// entity e's mass / moment of inertia / friction coefficients: the env's value where the world gives it per env,
+// else the compile-time constant
+template <class W, int e>
+DEVI float spec_mass(const SpecEnvParams<W>* p) {
+  if constexpr (SpecPerEnv<W>::at(e) & VMAS_F_MASS_ENV) return p->mass[e];
+  else return W::ent[e].mass;
+}
+template <class W, int e>
+DEVI float spec_inertia(const SpecEnvParams<W>* p) {
+  if constexpr (SpecPerEnv<W>::at(e) & VMAS_F_MASS_ENV) return p->inertia[e];
+  else return W::ent[e].inertia;
+}
+template <class W, int e>
+DEVI float spec_lin_fric(const SpecEnvParams<W>* p) {
+  if constexpr (SpecPerEnv<W>::at(e) & VMAS_F_LIN_FRIC_ENV) return p->lin_fric[e];
+  else return W::ent[e].lin_fric;
+}
+template <class W, int e>
+DEVI float spec_ang_fric(const SpecEnvParams<W>* p) {
+  if constexpr (SpecPerEnv<W>::at(e) & VMAS_F_ANG_FRIC_ENV) return p->ang_fric[e];
+  else return W::ent[e].ang_fric;
+}
+
 // Tuning knobs.  SPEC_BLOCK: threads (= envs) per block of the specialised kernels.
 // SPEC_MIN_BLOCKS: resident blocks per SM the register allocator must leave room for
 // (65536 / (SPEC_BLOCK * SPEC_MIN_BLOCKS) registers per thread at most).
@@ -528,9 +616,10 @@ DEVI void spec_trig(EnvRegs<E>& r) {
 }
 
 // action force / torque (clamped in place), friction, gravity of every entity -> r.Fx, r.Fy, r.T
-// (ref core.py:1995-2004, 2018-2102)
+// (ref core.py:1995-2004, 2018-2102).  `pe`: the env's per-env parameters (worlds with W::PER_ENV only)
 template <class W, int E, int NAX>
-DEVI void spec_entity_forces(EnvRegs<E>& r, float (&afx)[NAX], float (&afy)[NAX], float (&atq)[NAX]) {
+DEVI void spec_entity_forces(EnvRegs<E>& r, float (&afx)[NAX], float (&afy)[NAX], float (&atq)[NAX],
+                             const SpecEnvParams<W>* pe = nullptr) {
   constexpr float sub_dt = W::cfg.sub_dt;
   static_for<E>([&](auto ei) {
     constexpr int e = decltype(ei)::value;
@@ -565,26 +654,33 @@ DEVI void spec_entity_forces(EnvRegs<E>& r, float (&afx)[NAX], float (&afy)[NAX]
     if constexpr (en.flags & VMAS_F_LIN_FRIC) {
       const float speed = norm2(r.vx[e], r.vy[e]);
       if (speed != 0.f) {
-        const float cap = en.lin_fric * en.mass;
-        Fx = Fx + (-(r.vx[e] / speed)) * fminf(cap, (fabsf(r.vx[e]) / sub_dt) * en.mass);
-        Fy = Fy + (-(r.vy[e] / speed)) * fminf(cap, (fabsf(r.vy[e]) / sub_dt) * en.mass);
+        const float mass = spec_mass<W, e>(pe);
+        const float cap = spec_lin_fric<W, e>(pe) * mass;
+        Fx = Fx + (-(r.vx[e] / speed)) * fminf(cap, (fabsf(r.vx[e]) / sub_dt) * mass);
+        Fy = Fy + (-(r.vy[e] / speed)) * fminf(cap, (fabsf(r.vy[e]) / sub_dt) * mass);
       }
     }
     if constexpr (en.flags & VMAS_F_ANG_FRIC) {
       const float speed = sqrtf(r.w[e] * r.w[e]);
       if (speed != 0.f) {
-        const float cap = en.ang_fric * en.inertia;
-        T = T + (-(r.w[e] / speed)) * fminf(cap, (fabsf(r.w[e]) / sub_dt) * en.inertia);
+        const float inertia = spec_inertia<W, e>(pe);
+        const float cap = spec_ang_fric<W, e>(pe) * inertia;
+        T = T + (-(r.w[e] / speed)) * fminf(cap, (fabsf(r.w[e]) / sub_dt) * inertia);
       }
     }
     if constexpr (en.flags & VMAS_F_MOVABLE) {
+      const float mass = spec_mass<W, e>(pe);
       if constexpr (W::cfg.has_world_gravity) {
-        Fx = Fx + en.mass * W::cfg.gravity_x;
-        Fy = Fy + en.mass * W::cfg.gravity_y;
+        Fx = Fx + mass * W::cfg.gravity_x;
+        Fy = Fy + mass * W::cfg.gravity_y;
       }
       if constexpr (en.flags & VMAS_F_GRAVITY) {
-        Fx = Fx + en.mass * en.grav_x;
-        Fy = Fy + en.mass * en.grav_y;
+        Fx = Fx + mass * en.grav_x;
+        Fy = Fy + mass * en.grav_y;
+      }
+      if constexpr (SpecPerEnv<W>::at(e) & VMAS_F_GRAVITY_ENV) {
+        Fx = Fx + mass * pe->gx[e];
+        Fy = Fy + mass * pe->gy[e];
       }
     }
     r.Fx[e] = Fx;
@@ -595,7 +691,7 @@ DEVI void spec_entity_forces(EnvRegs<E>& r, float (&afx)[NAX], float (&afy)[NAX]
 
 // semi-implicit Euler of every entity (ref core.py:2862-2908); `sub` is the substep's index in the step
 template <class W, int E>
-DEVI void spec_integrate(EnvRegs<E>& r, const int sub) {
+DEVI void spec_integrate(EnvRegs<E>& r, const int sub, const SpecEnvParams<W>* pe = nullptr) {
   constexpr float sub_dt = W::cfg.sub_dt;
   static_for<E>([&](auto ei) {
     constexpr int e = decltype(ei)::value;
@@ -605,8 +701,8 @@ DEVI void spec_integrate(EnvRegs<E>& r, const int sub) {
         r.vx[e] = r.vx[e] * en.drag_mult;
         r.vy[e] = r.vy[e] * en.drag_mult;
       }
-      r.vx[e] = r.vx[e] + div_pos(r.Fx[e], en.mass) * sub_dt;
-      r.vy[e] = r.vy[e] + div_pos(r.Fy[e], en.mass) * sub_dt;
+      r.vx[e] = r.vx[e] + div_pos(r.Fx[e], spec_mass<W, e>(pe)) * sub_dt;
+      r.vy[e] = r.vy[e] + div_pos(r.Fy[e], spec_mass<W, e>(pe)) * sub_dt;
       if constexpr (en.flags & VMAS_F_MAX_SPEED) {
         const float n = norm2(r.vx[e], r.vy[e]);
         if (n > en.max_speed) {
@@ -625,7 +721,7 @@ DEVI void spec_integrate(EnvRegs<E>& r, const int sub) {
     }
     if constexpr (en.flags & VMAS_F_ROTATABLE) {
       if (sub == 0) r.w[e] = r.w[e] * en.drag_mult;
-      r.w[e] = r.w[e] + div_pos(r.T[e], en.inertia) * sub_dt;
+      r.w[e] = r.w[e] + div_pos(r.T[e], spec_inertia<W, e>(pe)) * sub_dt;
       r.rot[e] = r.rot[e] + r.w[e] * sub_dt;
     }
   });
@@ -934,13 +1030,15 @@ DEVI void spec_env_step(const SpecArgs& a, const long env, const uint32_t (&mask
   float afx[NA > 0 ? NA : 1], afy[NA > 0 ? NA : 1], atq[NA > 0 ? NA : 1];
   rows.unpack_pos_rot(r);
   rows.unpack_rest(r, afx, afy, atq);
+  SpecEnvParams<W> pe;
+  if constexpr (SpecPerEnv<W>::any) pe.load(a, env);
   uint32_t sig = 0;
   for (int sub = a.first_substep; sub < a.first_substep + a.n_substeps; ++sub) {
     spec_trig<W>(r);
-    spec_entity_forces<W>(r, afx, afy, atq);
+    spec_entity_forces<W>(r, afx, afy, atq, &pe);
     // joints and contacts, in accumulation order
     static_for<NI>([&](auto ii) { spec_item<W, decltype(ii)::value, TRACK>(r, a, env, mask_words, sig); });
-    spec_integrate<W>(r, sub);
+    spec_integrate<W>(r, sub, &pe);
   }
   rows.store(a, env, r, afx, afy, atq);
   if constexpr (!std::is_void_v<P>) {
@@ -992,6 +1090,7 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_spec_kernel(cons
 // The whole-step kernel: step_spec_kernel with the epilogue P behind the last substep.
 template <class W, class P>
 __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_fused_kernel(const SpecArgs a, const EpiArgs e) {
+  static_assert(!SpecPerEnv<W>::any, "no whole-step kernel for worlds with per-env parameters");
   constexpr int MW = W::MASK_WORDS;
   const long tid = (long)blockIdx.x * W::BLOCK + threadIdx.x;
   uint32_t mask_words[MW > 0 ? MW : 1];
@@ -1082,6 +1181,7 @@ DEVI ItemOut spec_round_swap(const ItemOut& o) {
 template <class W, class P, int G>
 __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_BLOCKS / G : 1))
     step_env_kernel(const SpecArgs a, const EpiArgs e, const ActArgs act) {
+  static_assert(!SpecPerEnv<W>::any, "no whole-step kernel for worlds with per-env parameters");
   constexpr int MW = W::MASK_WORDS, E = W::E, NA = W::A;
   using R = SpecRounds<W, G>;
   const long tid = ((long)blockIdx.x * (W::BLOCK * G) + threadIdx.x) / G;
@@ -1288,6 +1388,12 @@ static cudaError_t launch_fused(const SpecArgs& a, const EpiArgs& e, cudaStream_
 // host-side launcher used by the registry in generated/specializations.cuh
 template <class W>
 static cudaError_t launch_spec(const SpecArgs& a, cudaStream_t stream) {
+  if constexpr (spec_needs_params<W>()) {
+    if (!a.ent_params) return cudaErrorInvalidValue;  // (a world with per-env mass / friction needs its table)
+  }
+  if constexpr (spec_needs_gravity<W>()) {
+    if (!a.ent_gravity) return cudaErrorInvalidValue;
+  }
   const long blocks = ((long)a.batch_dim + W::BLOCK - 1) / W::BLOCK;
   if (a.order || a.sig)
     step_spec_kernel<W, true><<<(unsigned)blocks, W::BLOCK, 0, stream>>>(a);

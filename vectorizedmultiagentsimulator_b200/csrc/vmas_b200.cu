@@ -51,7 +51,20 @@ struct StepArgs {
   int mask_words;
   int first_substep;
   int n_substeps;
+  const float* ent_params = nullptr;  // [B, E, VMAS_EP_COLS] per-env mass / friction of flagged entities, or null
 };
+
+// an entity's per-env parameter (VMAS_F_*_ENV flag `bit`, column `col` of ent_params) or its scalar column
+DEVI float ent_param(const StepArgs& a, int flg, int bit, long env, int e, int col, const float* ef, int ef_col) {
+  return ((flg & bit) && a.ent_params) ? a.ent_params[((size_t)env * a.cfg.n_entities + e) * VMAS_EP_COLS + col]
+                                       : __ldg(ef + ef_col);
+}
+// moment of inertia: per env from the env's mass (VMAS_F_MASS_ENV), else the scalar column
+DEVI float ent_inertia(const StepArgs& a, int flg, float mass, const float* ef) {
+  return ((flg & VMAS_F_MASS_ENV) && a.ent_params)
+             ? (__ldg(ef + VMAS_EF_INERTIA_K0) * mass) * __ldg(ef + VMAS_EF_INERTIA_K1)
+             : __ldg(ef + VMAS_EF_INERTIA);
+}
 
 // ---------------------------------------------------------------------------------------------
 // per-entity geometry cached in shared memory for the work-item phase
@@ -332,7 +345,7 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
           sh.s2[e] = sn;
         }
       }
-      const float mass = __ldg(ef + VMAS_EF_MASS);
+      const float mass = ent_param(a, flg[j], VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS);
       if (flg[j] & VMAS_F_AGENT) {  // ref core.py:2018-2041
         if (flg[j] & VMAS_F_MOVABLE) {
           if (flg[j] & VMAS_F_MAX_F) {
@@ -367,7 +380,7 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
       if (flg[j] & VMAS_F_LIN_FRIC) {  // ref core.py:2054-2088
         const float speed = norm2(vx[j], vy[j]);
         if (speed != 0.f) {
-          const float cap = __ldg(ef + VMAS_EF_LIN_FRIC) * mass;
+          const float cap = ent_param(a, flg[j], VMAS_F_LIN_FRIC_ENV, env, e, VMAS_EP_LIN_FRIC, ef, VMAS_EF_LIN_FRIC) * mass;
           Fx[j] = Fx[j] + (-(vx[j] / speed)) * fminf(cap, (fabsf(vx[j]) / sub_dt) * mass);
           Fy[j] = Fy[j] + (-(vy[j] / speed)) * fminf(cap, (fabsf(vy[j]) / sub_dt) * mass);
         }
@@ -375,8 +388,8 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
       if (flg[j] & VMAS_F_ANG_FRIC) {  // ref core.py:2089-2102
         const float speed = sqrtf(w[j] * w[j]);
         if (speed != 0.f) {
-          const float inertia = __ldg(ef + VMAS_EF_INERTIA);
-          const float cap = __ldg(ef + VMAS_EF_ANG_FRIC) * inertia;
+          const float inertia = ent_inertia(a, flg[j], mass, ef);
+          const float cap = ent_param(a, flg[j], VMAS_F_ANG_FRIC_ENV, env, e, VMAS_EP_ANG_FRIC, ef, VMAS_EF_ANG_FRIC) * inertia;
           T[j] = T[j] + (-(w[j] / speed)) * fminf(cap, (fabsf(w[j]) / sub_dt) * inertia);
         }
       }
@@ -444,7 +457,7 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
       const float* ef = a.tb.ent_f32 + (size_t)e * VMAS_EF_COLS;
       const float drag_mult = __ldg(ef + VMAS_EF_DRAG_MULT);
       if (movable) {
-        const float mass = __ldg(ef + VMAS_EF_MASS);
+        const float mass = ent_param(a, flg[j], VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS);
         if (sub == 0) {
           vx[j] = vx[j] * drag_mult;
           vy[j] = vy[j] * drag_mult;
@@ -470,7 +483,8 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
         if (a.cfg.has_y_semidim) py[j] = fminf(fmaxf(py[j], -a.cfg.y_semidim), a.cfg.y_semidim);
       }
       if (rotatable) {
-        const float inertia = __ldg(ef + VMAS_EF_INERTIA);
+        const float inertia =
+            ent_inertia(a, flg[j], ent_param(a, flg[j], VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS), ef);
         if (sub == 0) w[j] = w[j] * drag_mult;
         w[j] = w[j] + div_pos(T[j], inertia) * sub_dt;
         rt[j] = rt[j] + w[j] * sub_dt;
@@ -587,7 +601,7 @@ __global__ void __launch_bounds__(BLOCK) step_tpe_kernel(const StepArgs a) {
         }
       }
       float Fx = 0.f, Fy = 0.f, T = 0.f;
-      const float mass = __ldg(ef + VMAS_EF_MASS);
+      const float mass = ent_param(a, flg, VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS);
       if (flg & VMAS_F_AGENT) {  // ref core.py:2018-2041
         const int ai = __ldg(a.tb.ent_i32 + e * 4 + 2);
         if (flg & VMAS_F_MOVABLE) {
@@ -632,7 +646,7 @@ __global__ void __launch_bounds__(BLOCK) step_tpe_kernel(const StepArgs a) {
         const float vx = TF(T_VX, e), vy = TF(T_VY, e);
         const float speed = norm2(vx, vy);
         if (speed != 0.f) {
-          const float cap = __ldg(ef + VMAS_EF_LIN_FRIC) * mass;
+          const float cap = ent_param(a, flg, VMAS_F_LIN_FRIC_ENV, env, e, VMAS_EP_LIN_FRIC, ef, VMAS_EF_LIN_FRIC) * mass;
           Fx = Fx + (-(vx / speed)) * fminf(cap, (fabsf(vx) / sub_dt) * mass);
           Fy = Fy + (-(vy / speed)) * fminf(cap, (fabsf(vy) / sub_dt) * mass);
         }
@@ -641,8 +655,8 @@ __global__ void __launch_bounds__(BLOCK) step_tpe_kernel(const StepArgs a) {
         const float w = TF(T_W, e);
         const float speed = sqrtf(w * w);
         if (speed != 0.f) {
-          const float inertia = __ldg(ef + VMAS_EF_INERTIA);
-          const float cap = __ldg(ef + VMAS_EF_ANG_FRIC) * inertia;
+          const float inertia = ent_inertia(a, flg, mass, ef);
+          const float cap = ent_param(a, flg, VMAS_F_ANG_FRIC_ENV, env, e, VMAS_EP_ANG_FRIC, ef, VMAS_EF_ANG_FRIC) * inertia;
           T = T + (-(w / speed)) * fminf(cap, (fabsf(w) / sub_dt) * inertia);
         }
       }
@@ -695,7 +709,7 @@ __global__ void __launch_bounds__(BLOCK) step_tpe_kernel(const StepArgs a) {
       const float* ef = a.tb.ent_f32 + (size_t)e * VMAS_EF_COLS;
       const float drag_mult = __ldg(ef + VMAS_EF_DRAG_MULT);
       if (flg & VMAS_F_MOVABLE) {
-        const float mass = __ldg(ef + VMAS_EF_MASS);
+        const float mass = ent_param(a, flg, VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS);
         float vx = TF(T_VX, e), vy = TF(T_VY, e);
         if (sub == 0) {
           vx = vx * drag_mult;
@@ -726,7 +740,8 @@ __global__ void __launch_bounds__(BLOCK) step_tpe_kernel(const StepArgs a) {
         TF(T_PY, e) = py;
       }
       if (flg & VMAS_F_ROTATABLE) {
-        const float inertia = __ldg(ef + VMAS_EF_INERTIA);
+        const float inertia =
+            ent_inertia(a, flg, ent_param(a, flg, VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS), ef);
         float w = TF(T_W, e);
         if (sub == 0) w = w * drag_mult;
         w = w + div_pos(TF(T_TQ, e), inertia) * sub_dt;
@@ -1751,6 +1766,8 @@ static SpecArgs spec_args_of(const StepArgs& args) {
   sa.n_substeps = args.n_substeps;
   sa.order = nullptr;
   sa.sig = nullptr;
+  sa.ent_params = args.ent_params;
+  sa.ent_gravity = args.tb.ent_gravity;
   return sa;
 }
 
@@ -1777,6 +1794,8 @@ static int dispatch_spec(const StepArgs& args, cudaStream_t stream) {
   sa.n_substeps = args.n_substeps;
   sa.order = args.tb.env_order;
   sa.sig = args.tb.env_signature;
+  sa.ent_params = args.ent_params;
+  sa.ent_gravity = args.tb.ent_gravity;
   // tb.group selects the thread mapping of a specialised world: 1 = one thread per env,
   // VMAS_GROUP_TILE = a warp owns a tile of 32 envs and runs the narrow phase compacted
   if (args.tb.group == VMAS_GROUP_TILE) {
@@ -1935,7 +1954,7 @@ const char* vmas_b200_last_error(void) { return g_last_error; }
 static int substeps_impl(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,
                          uint32_t* mask, int exact_broad_phase, int first_substep, int n_substeps,
                          void* cuda_stream, void* ev_begin, void* ev_end, int fused = 0,
-                         const EpiArgs* epi = nullptr) {
+                         const EpiArgs* epi = nullptr, const float* ent_params = nullptr) {
   if (check_common(cfg, tb, st) < 0) return -1;
   if (cfg->n_agents > 0 && (!st->force || !st->torque)) return fail("null force/torque pointer%s");
   if (cfg->n_items > 0 && (!tb->item_f32 || !tb->item_i32 || !tb->sched || !tb->inc || !tb->inc_off))
@@ -1948,6 +1967,7 @@ static int substeps_impl(const VmasWorldConfig* cfg, const VmasPlanTables* tb, c
   args.st = *st;
   args.mask = mask;
   args.mask_words = (cfg->n_masked + 31) / 32;
+  args.ent_params = ent_params;
   const bool masked = cfg->n_masked > 0 && exact_broad_phase;
   if (masked && (!mask || !tb->masked_items)) return fail("broad-phase mask scratch missing%s");
   int launches = 0;
@@ -1994,10 +2014,16 @@ int vmas_b200_world_step_timed(const VmasWorldConfig* cfg, const VmasPlanTables*
   return substeps_impl(cfg, tb, st, mask, exact_broad_phase, 0, cfg->substeps, cuda_stream, ev_begin, ev_end);
 }
 
+int vmas_b200_world_step_params(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const float* ent_params,
+                                const VmasState* st, uint32_t* mask, int exact_broad_phase, void* cuda_stream) {
+  if (!cfg) return fail("null argument%s");
+  return substeps_impl(cfg, tb, st, mask, exact_broad_phase, 0, cfg->substeps, cuda_stream, nullptr, nullptr, 0,
+                       nullptr, ent_params);
+}
+
 int vmas_b200_world_step(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,
                          uint32_t* mask, int exact_broad_phase, void* cuda_stream) {
-  if (!cfg) return fail("null argument%s");
-  return vmas_b200_world_substeps(cfg, tb, st, mask, exact_broad_phase, 0, cfg->substeps, cuda_stream);
+  return vmas_b200_world_step_params(cfg, tb, nullptr, st, mask, exact_broad_phase, cuda_stream);
 }
 
 int vmas_b200_broad_phase(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,

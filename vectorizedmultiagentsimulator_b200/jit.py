@@ -43,10 +43,16 @@ namespace vmas {{
 }}  // namespace vmas
 
 using W = vmas::{name};
+// no tile kernel for a world with per-env parameters (it steps on step_spec_kernel)
+template <class X>
+cudaError_t jit_launch_tile(const vmas::SpecArgs& a, cudaStream_t stream) {{
+  if constexpr (vmas::SpecPerEnv<X>::any) return cudaErrorNotSupported;
+  else return vmas::launch_tile<X>(a, stream);
+}}
 extern "C" {{
 cudaError_t vmas_jit_launch(const vmas::SpecArgs& a, cudaStream_t stream) {{ return vmas::launch_spec<W>(a, stream); }}
-cudaError_t vmas_jit_launch_tile(const vmas::SpecArgs& a, cudaStream_t stream) {{ return vmas::launch_tile<W>(a, stream); }}
-int vmas_jit_has_tile(void) {{ return vmas::TileLayout<W>::SUPPORTED ? 1 : 0; }}
+cudaError_t vmas_jit_launch_tile(const vmas::SpecArgs& a, cudaStream_t stream) {{ return jit_launch_tile<W>(a, stream); }}
+int vmas_jit_has_tile(void) {{ return vmas::TileLayout<W>::SUPPORTED && !vmas::SpecPerEnv<W>::any ? 1 : 0; }}
 int vmas_jit_spec_args_bytes(void) {{ return (int)sizeof(vmas::SpecArgs); }}
 }}
 """
@@ -166,8 +172,8 @@ def available() -> bool:
 
 def request(desc: P.WorldDescription) -> Optional[Job]:
     """Starts (or finds) the compilation of ``desc``'s specialisation; None if the world cannot be
-    specialised (too large, per-env gravity tensors) or the JIT is off / has no compiler."""
-    if not available() or not codegen.specializable(desc):
+    specialised (too large) or the JIT is off / has no compiler."""
+    if not available() or not codegen.specializable(desc, per_env=True):
         return None
     h = codegen.world_hash(desc)
     with _lock:
@@ -220,7 +226,8 @@ _step_jobs: Dict[int, StepKernelJob] = {}
 
 
 def request_step_kernel(desc: P.WorldDescription, cols, instrs, acts=(), block: bool = False) -> Optional[StepKernelJob]:
-    """Starts (or finds) the compilation of the whole-step kernel; None if the world cannot be specialised.
+    """Starts (or finds) the compilation of the whole-step kernel; None if the world cannot be specialised or
+    has per-env physical parameters (those step on the captured graph of the specialised substep kernel).
     ``acts``: [(agent row, u_range x 2, u_multiplier x 2)] of the policy agents if the kernel is to ingest
     their (continuous, holonomic) actions itself."""
     if not available() or not codegen.specializable(desc):

@@ -91,6 +91,10 @@ class VelocityController:
         return True
 
     def process_force(self):
+        if isinstance(self.agent.mass, torch.Tensor) and self.agent.mass.dim() > 0:
+            raise NotImplementedError(
+                f"Entity '{self.agent.name}': a per-env mass on an agent driven by the velocity controller is out of scope"
+            )
         if self._process_force_cuda():
             return
         self.accum_errs = self.accum_errs.to(self.world.device)

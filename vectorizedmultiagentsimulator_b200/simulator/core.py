@@ -414,6 +414,27 @@ class Action(TorchVectorizedObject):
                 setattr(self, name, t.to(device))
 
 
+#: physical parameters an entity may hold per env, as a [batch_dim, 1] fp32 tensor (domain randomisation)
+PER_ENV_PARAMS = ("mass", "linear_friction", "angular_friction")
+
+
+def _is_param_tensor(value) -> bool:
+    return isinstance(value, Tensor) and value.dim() > 0
+
+
+def _checked_param(entity_name: str, attr: str, value):
+    """``value`` if it is a python number, None, a 0-d tensor or a 2-D ``[n, 1]`` fp32 tensor; else ValueError.
+    (The batch size and the device are checked once the entity belongs to a world.)"""
+    if value is None or isinstance(value, (int, float)) or not _is_param_tensor(value):
+        return value
+    if value.dtype != torch.float32 or value.dim() != 2 or value.shape[1] != 1:
+        raise ValueError(
+            f"Entity '{entity_name}': {attr} must be a python number or a float32 tensor of shape "
+            f"[batch_dim, 1], got {value.dtype} {list(value.shape)}"
+        )
+    return value.detach().clone()
+
+
 # ----------------------------------------------------------------------------------------
 # Entities (ref core.py:538-1086)
 # ----------------------------------------------------------------------------------------
@@ -444,7 +465,7 @@ class Entity(TorchVectorizedObject, Observable, ABC):
         self._rotatable = rotatable
         self._collide = collide
         self._density = density
-        self._mass = mass
+        self._mass = _checked_param(name, "mass", mass)
         self._max_speed = max_speed
         self._v_range = v_range
         self._color = color
@@ -453,8 +474,8 @@ class Entity(TorchVectorizedObject, Observable, ABC):
         self._collision_filter = collision_filter
         self._state = EntityState()
         self._drag = drag
-        self._linear_friction = linear_friction
-        self._angular_friction = angular_friction
+        self._linear_friction = _checked_param(name, "linear_friction", linear_friction)
+        self._angular_friction = _checked_param(name, "angular_friction", angular_friction)
         if gravity is None or isinstance(gravity, Tensor):
             self._gravity = gravity
         else:
@@ -472,6 +493,40 @@ class Entity(TorchVectorizedObject, Observable, ABC):
     def batch_dim(self, batch_dim: int):
         TorchVectorizedObject.batch_dim.fset(self, batch_dim)
         self._state.batch_dim = batch_dim
+        for attr in PER_ENV_PARAMS:  # a tensor given to the constructor meets its world's batch here
+            value = getattr(self, "_" + attr)
+            if _is_param_tensor(value) and batch_dim is not None and value.shape[0] != batch_dim:
+                raise ValueError(
+                    f"Entity '{self.name}': {attr} must be a float32 tensor of shape [batch_dim, 1] = "
+                    f"[{batch_dim}, 1], got {list(value.shape)}"
+                )
+
+    def _set_param(self, attr: str, value):
+        """Setter of a per-env-capable physical parameter (mass, linear / angular friction).
+
+        A python number is structure, as before: the plan is rebuilt.  A ``[batch_dim, 1]`` fp32 tensor on the
+        world's device is copied into a buffer the entity owns (allocated on the first tensor assignment and
+        kept while the attribute stays a tensor), so a tensor after a tensor is data only: no plan rebuild and
+        a captured CUDA graph keeps reading the same address."""
+        value = _checked_param(self.name, attr, value)
+        old = getattr(self, "_" + attr)
+        if _is_param_tensor(value):
+            if self.batch_dim is not None and value.shape[0] != self.batch_dim:
+                raise ValueError(
+                    f"Entity '{self.name}': {attr} must be a float32 tensor of shape [batch_dim, 1] = "
+                    f"[{self.batch_dim}, 1], got {list(value.shape)}"
+                )
+            want = None if self.device is None else torch.device(self.device)
+            if want is not None and (value.device.type != want.type or want.index not in (None, value.device.index)):
+                raise ValueError(f"Entity '{self.name}': {attr} must be on the world's device {want}, got {value.device}")
+            if _is_param_tensor(old) and old.shape == value.shape and old.device == value.device:
+                if value.data_ptr() != old.data_ptr():
+                    old.copy_(value)
+                return
+            setattr(self, "_" + attr, value.detach().clone())
+        else:
+            setattr(self, "_" + attr, value)
+        self._touch()
 
     @property
     def is_rendering(self):
@@ -497,9 +552,8 @@ class Entity(TorchVectorizedObject, Observable, ABC):
         return self._mass
 
     @mass.setter
-    def mass(self, mass: float):
-        self._mass = mass
-        self._touch()
+    def mass(self, mass):
+        self._set_param("mass", mass)
 
     @property
     def moment_of_inertia(self):
@@ -565,12 +619,15 @@ class Entity(TorchVectorizedObject, Observable, ABC):
 
     @linear_friction.setter
     def linear_friction(self, value):
-        self._linear_friction = value
-        self._touch()
+        self._set_param("linear_friction", value)
 
     @property
     def angular_friction(self):
         return self._angular_friction
+
+    @angular_friction.setter
+    def angular_friction(self, value):
+        self._set_param("angular_friction", value)
 
     @property
     def gravity(self):

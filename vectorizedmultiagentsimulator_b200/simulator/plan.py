@@ -47,6 +47,10 @@ F_MAX_T = 1 << 11
 F_T_RANGE = 1 << 12
 F_TRIG = 1 << 13  # kernel must evaluate sin/cos of this entity's rotation
 F_GRAVITY_ENV = 1 << 14  # per-env gravity rows in ent_gravity[B, E, 2]
+F_MASS_ENV = 1 << 15  # per-env mass in ent_params[B, E, 4] column 0 (moment of inertia derived in the kernel)
+F_LIN_FRIC_ENV = 1 << 16  # per-env linear-friction coefficient, ent_params column 1
+F_ANG_FRIC_ENV = 1 << 17  # per-env angular-friction coefficient, ent_params column 2
+F_PARAMS_ENV = F_MASS_ENV | F_LIN_FRIC_ENV | F_ANG_FRIC_ENV
 
 # columns of ent_f32
 (
@@ -67,8 +71,15 @@ F_GRAVITY_ENV = 1 << 14  # per-env gravity rows in ent_gravity[B, E, 2]
     EF_T_RANGE,
     EF_CIRC_R,
     EF_R_PLUS_LMD,
-) = range(17)
+    EF_INERTIA_K0,
+    EF_INERTIA_K1,
+) = range(19)
 EF_COLS = 20
+#: columns of the per-env parameter table ent_params[B, E, EP_COLS]
+EP_MASS, EP_LIN_FRIC, EP_ANG_FRIC = 0, 1, 2
+EP_COLS = 4
+#: what a per-env attribute's scalar field holds in a description: the hash does not see the values
+PER_ENV_PLACEHOLDER = 1.0
 EI_COLS = 4  # shape kind, flags, agent index, reserved
 
 # columns of item_f32 / item_i32
@@ -93,6 +104,35 @@ def _shape_kind(shape) -> int:
 
 def _is_agent(entity) -> bool:
     return hasattr(entity, "action") and hasattr(entity, "dynamics")
+
+
+#: action models that back-solve the force / torque from the agent's mass in the action ingest
+KINEMATIC_DYNAMICS = ("DiffDrive", "KinematicBicycle", "Drone")
+
+
+def _is_per_env(entity, attr) -> bool:
+    """True if ``entity.<attr>`` is a ``[batch_dim, 1]`` tensor (mass, linear / angular friction)."""
+    v = getattr(entity, attr, None)
+    if v is None or isinstance(v, (int, float)):
+        return False
+    if hasattr(v, "dim") and v.dim() == 0:
+        return False
+    if hasattr(v, "shape") and v.dim() == 2 and v.shape[1] == 1:
+        return True
+    raise NotImplementedError(
+        f"Entity '{entity.name}': {attr} must be a python number or a [batch_dim, 1] tensor, got shape "
+        f"{tuple(getattr(v, 'shape', ()))}"
+    )
+
+
+def inertia_constants(shape_kind: int, d0: float, d1: float):
+    """(K0, K1) with moment_of_inertia(m) = fl(fl(K0 * m) * K1) for a per-env fp32 mass ``m``: the
+    python-double factors of ref core.py:123-124, 160-161, 187-188, each rounded once to fp32."""
+    if shape_kind == SHAPE_SPHERE:
+        return 1 / 2, d0**2
+    if shape_kind == SHAPE_BOX:
+        return 1 / 12, d0**2 + d1**2
+    return 1 / 12, d0**2
 
 
 def _as_pair(value):
@@ -162,12 +202,16 @@ def describe_entity(entity, agent_index: int) -> Dict:
         raise NotImplementedError(
             f"Entity '{entity.name}': gravity must be a scalar, an (x, y) pair or a [batch_dim, 2] tensor"
         )
-    for attr in ("linear_friction", "angular_friction"):
+    per_env = {attr: _is_per_env(entity, attr) for attr in ("mass", "linear_friction", "angular_friction")}
+    if per_env["mass"] and type(getattr(entity, "dynamics", None)).__name__ in KINEMATIC_DYNAMICS:
+        raise NotImplementedError(
+            f"Entity '{entity.name}': a per-env mass on an agent whose action model reads the mass "
+            f"({type(entity.dynamics).__name__}) is out of scope; give it a scalar mass"
+        )
+
+    def scalar(attr):
         v = getattr(entity, attr, None)
-        if v is not None and not isinstance(v, (int, float)):
-            raise NotImplementedError(
-                f"Entity '{entity.name}' has a tensor-valued {attr}; the CUDA kernels take a scalar"
-            )
+        return None if v is None else (PER_ENV_PLACEHOLDER if per_env[attr] else float(v))
 
     def opt(name):
         v = getattr(entity, name, None) if (is_agent or name in ("v_range", "max_speed")) else None
@@ -183,13 +227,16 @@ def describe_entity(entity, agent_index: int) -> Dict:
         hollow=hollow,
         movable=bool(entity.movable),
         rotatable=bool(entity.rotatable),
-        mass=float(entity.mass),
-        inertia=float(entity.moment_of_inertia),
+        mass=scalar("mass"),
+        inertia=PER_ENV_PLACEHOLDER if per_env["mass"] else float(entity.moment_of_inertia),
         drag=None if entity.drag is None else float(entity.drag),
-        linear_friction=None if entity.linear_friction is None else float(entity.linear_friction),
-        angular_friction=None if entity.angular_friction is None else float(entity.angular_friction),
+        linear_friction=scalar("linear_friction"),
+        angular_friction=scalar("angular_friction"),
         gravity=None if gravity_pair is None else list(gravity_pair),
         gravity_per_env=bool(gravity_per_env),
+        mass_per_env=per_env["mass"],
+        lin_fric_per_env=per_env["linear_friction"],
+        ang_fric_per_env=per_env["angular_friction"],
         max_speed=opt("max_speed"),
         v_range=opt("v_range"),
         max_f=opt("max_f"),
@@ -361,6 +408,13 @@ def build_tables(desc: WorldDescription) -> PlanTables:
             row[EF_GRAV_X], row[EF_GRAV_Y] = e["gravity"]
         if e.get("gravity_per_env"):
             flags |= F_GRAVITY_ENV
+        if e.get("mass_per_env"):
+            flags |= F_MASS_ENV
+            row[EF_INERTIA_K0], row[EF_INERTIA_K1] = inertia_constants(e["shape"], e["d0"], e["d1"])
+        if e.get("lin_fric_per_env"):
+            flags |= F_LIN_FRIC_ENV
+        if e.get("ang_fric_per_env"):
+            flags |= F_ANG_FRIC_ENV
         for name, col, bit in (
             ("max_speed", EF_MAX_SPEED, F_MAX_SPEED),
             ("v_range", EF_V_RANGE, F_V_RANGE),
