@@ -370,8 +370,9 @@ int vmas_b200_point_query(const VmasWorldConfig* cfg, const VmasPlanTables* tb, 
  *   dyn_params   [0] dt  [1] mass  [2] moment of inertia  [3] 1 = RK4, 0 = Euler;
  *                bicycle: [4] l_f  [5] l_r  [6] max steering angle;  drone: [4] I_xx  [5] I_yy  [6] I_zz  [7] g
  *   dyn_state    drone only: device fp32 [B, 12] (roll pitch yaw | p q r | vx vy vz | x y z), updated in place
- *   bad_flag     device uint8[1] or NULL: set to 1 if any action is NaN or outside +-u_range
- *                (the reference asserts; here the host reads the flag back asynchronously)
+ *   bad_flag     device uint8[1] or NULL: set to 1 if any action is NaN (with or without `clamp`: a NaN passes
+ *                the clamp unchanged) or outside +-u_range after the optional clamp (the reference asserts;
+ *                here the host reads the flag back asynchronously)
  */
 #define VMAS_MAX_INGEST_AGENTS 16
 #define VMAS_MAX_ACTION_SIZE 8

@@ -41,6 +41,8 @@ SOURCES = [os.path.join(CSRC, "vmas_b200.cu")]
 GENERATED = os.path.join(CSRC, "generated", "specializations.cuh")
 HEADERS = [
     os.path.join(CSRC, "geometry.cuh"),
+    os.path.join(CSRC, "query.cuh"),
+    os.path.join(CSRC, "ingest.cuh"),
     os.path.join(CSRC, "spec_kernel.cuh"),
     os.path.join(CSRC, "spec_tile_kernel.cuh"),
     os.path.join(CSRC, "reset.cuh"),

@@ -17,6 +17,7 @@
 #include <utility>
 
 #include "geometry.cuh"
+#include "ingest.cuh"
 #include "query.cuh"
 #include "vmas_b200.h"
 
@@ -1206,13 +1207,9 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
     constexpr ActC c0 = P::act[k0], c1 = P::act[k1];
     const bool o = k0 != k1 && odd;
     const float range0 = o ? c1.range0 : c0.range0, range1 = o ? c1.range1 : c0.range1;
-    float2 v = reinterpret_cast<const float2*>(o ? act.actions[k1] : act.actions[k0])[env];
-    if (act.clamp) {  // torch.clamp keeps NaN
-      v.x = fminf(fmaxf(v.x, -range0), range0);
-      v.y = fminf(fmaxf(v.y, -range1), range1);
-    }
-    bad |= (v.x != v.x) || (fabsf(v.x) > range0) || (v.y != v.y) || (fabsf(v.y) > range1);
-    const float2 u = make_float2(v.x * (o ? c1.mult0 : c0.mult0), v.y * (o ? c1.mult1 : c0.mult1));
+    const float2 v = reinterpret_cast<const float2*>(o ? act.actions[k1] : act.actions[k0])[env];
+    const float ux = ingest_continuous(v.x, range0, o ? c1.mult0 : c0.mult0, act.clamp, bad);
+    const float2 u = make_float2(ux, ingest_continuous(v.y, range1, o ? c1.mult1 : c0.mult1, act.clamp, bad));
     if (live && (k0 != k1 || !odd)) reinterpret_cast<float2*>(o ? act.u[k1] : act.u[k0])[env] = u;
     if constexpr (k0 == k1) {
       afx[c0.agent] = u.x;

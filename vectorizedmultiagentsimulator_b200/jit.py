@@ -93,7 +93,7 @@ _keepalive = []  # loaded objects must outlive the registry entries that point i
 def _source_stamp() -> str:
     """Hash of the headers the object is compiled from: a header edit invalidates the cache."""
     h = hashlib.sha1()
-    for name in ("geometry.cuh", "query.cuh", "spec_kernel.cuh", "spec_tile_kernel.cuh"):
+    for name in ("geometry.cuh", "query.cuh", "ingest.cuh", "spec_kernel.cuh", "spec_tile_kernel.cuh"):
         h.update(open(os.path.join(_native.CSRC, name), "rb").read())
     h.update(open(os.path.join(_native.INCLUDE, "vmas_b200.h"), "rb").read())
     return h.hexdigest()[:12]
