@@ -93,7 +93,8 @@ typedef struct VmasPlanTables {
   int32_t group;              /* lanes per env: 1 = one thread per env (default), or 8, 16, 32; with a
                                  specialization: 1, or VMAS_GROUP_TILE = the warp-tile kernel (a warp owns
                                  32 envs; far tests per env, then the narrow phase of the near (item, env)
-                                 pairs compacted over the warp's lanes; see csrc/spec_tile_kernel.cuh) */
+                                 pairs compacted over the warp's lanes; see csrc/spec_tile_kernel.cuh);
+                                 without one: VMAS_GROUP_BLOCK = a thread block per env (step_block_kernel) */
   int32_t ents_per_lane;      /* 1, 2 or 4 (E <= group * ents_per_lane) */
   int32_t specialization;     /* index from vmas_b200_find_specialization(), or -1: generic kernels */
   /* env scheduling of the specialised thread-per-env kernel (both optional, may be NULL): */
@@ -102,6 +103,10 @@ typedef struct VmasPlanTables {
 } VmasPlanTables;
 
 #define VMAS_GROUP_TILE (-8)
+/* A thread block per env, its state in shared memory as [field][entity]: for worlds of up to
+ * VMAS_BLOCK_MAX_ENTITIES entities whose one-thread-per-env layout does not fit in shared memory. */
+#define VMAS_GROUP_BLOCK (-16)
+#define VMAS_BLOCK_MAX_ENTITIES 1024
 
 /* The state slab.  DEVICE pointers. */
 typedef struct VmasState {

@@ -41,6 +41,7 @@ SOURCES = [os.path.join(CSRC, "vmas_b200.cu")]
 GENERATED = os.path.join(CSRC, "generated", "specializations.cuh")
 HEADERS = [
     os.path.join(CSRC, "geometry.cuh"),
+    os.path.join(CSRC, "generic_step.cuh"),
     os.path.join(CSRC, "query.cuh"),
     os.path.join(CSRC, "ingest.cuh"),
     os.path.join(CSRC, "spec_kernel.cuh"),
@@ -192,6 +193,12 @@ DYN_NONE, DYN_HOLONOMIC, DYN_HOLONOMIC_ROT, DYN_FORWARD, DYN_ROTATION, DYN_DIFF_
 
 MAX_SPAWN = 64
 GROUP_TILE = -8  # VMAS_GROUP_TILE
+GROUP_BLOCK = -16  # VMAS_GROUP_BLOCK
+#: entities per env the CUDA backend steps (VMAS_BLOCK_MAX_ENTITIES: the block-per-env kernel's limit)
+MAX_ENTITIES = 1024
+#: opt-in shared memory per block of sm_90 (227 KB), taken for a device without properties (``cpu``)
+SM90_SHARED_OPTIN = 232448
+TPE_FIELDS, TPE_MIN_BLOCK = 13, 32  # step_tpe_kernel: [13 fields][E][BLOCK] fp32, BLOCK = 64 or 32
 #: env scheduling of the specialised thread-per-env kernel: the envs are re-sorted by their contact
 #: signature every this many World.step calls (0 = off: thread t always steps env t).  OFF by default:
 #: it halves the warp-instructions (1.8 k per 32 envs at 31 of 32 lanes active) but the scattered rows
@@ -407,6 +414,20 @@ def lane_layout(n_entities: int):
     raise NotImplementedError(f"{n_entities} entities per env exceed the kernel's limit of 128")
 
 
+def shared_optin_bytes(device) -> int:
+    """Opt-in shared memory per block of ``device`` (the sm_90 value for a non-CUDA device)."""
+    device = torch.device(device)
+    if device.type != "cuda":
+        return SM90_SHARED_OPTIN
+    return int(torch.cuda.get_device_properties(device).shared_memory_per_block_optin)
+
+
+def tpe_fits(tables: P.PlanTables, device) -> bool:
+    """Whether the thread-per-env kernel's smallest block (32 envs) holds an env's state and the mask words."""
+    state = TPE_FIELDS * tables.desc.n_entities * TPE_MIN_BLOCK * 4
+    return state + 4 * ((tables.n_masked + 31) // 32) <= shared_optin_bytes(device)
+
+
 def make_config(tables: P.PlanTables, batch_dim: Optional[int] = None) -> WorldConfig:
     d = tables.desc
     cfg = WorldConfig()
@@ -439,7 +460,11 @@ class DeviceTables:
         self.device = torch.device(device)
         desc = tables.desc
         mapping = mapping or os.environ.get("VMAS_B200_MAPPING", "auto")
-        assert mapping in ("auto", "specialized", "tile", "thread_per_env", "lanes_per_env"), mapping
+        assert mapping in ("auto", "specialized", "tile", "thread_per_env", "lanes_per_env", "block_per_env"), mapping
+        if desc.n_entities > MAX_ENTITIES:
+            raise NotImplementedError(
+                f"{desc.n_entities} entities per env exceed the CUDA backend's limit of {MAX_ENTITIES}"
+            )
         self.specialization = -1
         # specialised worlds have two kernels: "specialized" = one thread per env (step_spec_kernel),
         # "tile" = a warp per 32 envs with the narrow phase compacted (step_tile_kernel; not for
@@ -452,7 +477,7 @@ class DeviceTables:
             if self.specialization < 0:
                 if mapping != "auto":
                     raise RuntimeError("no ahead-of-time specialisation of this world in libvmas_b200.so")
-                mapping = "thread_per_env"
+                mapping = "thread_per_env" if tpe_fits(tables, self.device) else "block_per_env"
             else:
                 has_tile = bool(lib.vmas_b200_specialization_has_tile(self.specialization))
                 if mapping == "tile" and not has_tile:
@@ -460,8 +485,9 @@ class DeviceTables:
                 if mapping == "auto":
                     mapping = "tile" if (has_tile and DEFAULT_SPEC_MAPPING == "tile") else "specialized"
         self.mapping = mapping
-        if mapping in ("thread_per_env", "specialized", "tile"):
-            self.group, self.ents_per_lane = (GROUP_TILE if mapping == "tile" else 1), desc.n_entities
+        if mapping in ("thread_per_env", "specialized", "tile", "block_per_env"):
+            group = {"tile": GROUP_TILE, "block_per_env": GROUP_BLOCK}.get(mapping, 1)
+            self.group, self.ents_per_lane = group, desc.n_entities
             sched = np.zeros((0, 1), np.int32)
         else:
             self.group, self.ents_per_lane = lane_layout(desc.n_entities)

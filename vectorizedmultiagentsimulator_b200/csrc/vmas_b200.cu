@@ -8,6 +8,8 @@
 //                         memory and summed per entity in the reference's order (deterministic,
 //                         no atomics).  Sphere-only worlds run all substeps in one launch with
 //                         the state held in registers.
+//   step_tpe_kernel       the same substeps with one thread per env, its state in shared memory.
+//   step_block_kernel     the same substeps with one block per env, for worlds of up to 1024 entities.
 //   broad_phase_kernel    batch-wide activation mask of line/box pairs (ref core.py:2797-2801).
 //   cast_rays_kernel      LIDAR: thread per (env, ray), min over target entities.
 //   pair_query_kernel /   World.get_distance / is_overlapping / get_distance_from_point.
@@ -20,6 +22,7 @@
 #include <string.h>
 
 #include "geometry.cuh"
+#include "generic_step.cuh"
 #include "query.cuh"
 #include "ingest.cuh"
 #include "generated/specializations.cuh"
@@ -39,208 +42,6 @@ static int fail(const char* fmt, const char* detail = "") {
     cudaError_t _e = (expr);                                             \
     if (_e != cudaSuccess) return fail("CUDA error: %s", cudaGetErrorString(_e)); \
   } while (0)
-
-constexpr float HALF_PI_F = 1.57079632679489661923f;  // fp32(torch.pi / 2)
-constexpr float LINE_MIN_DIST_F = (float)(4.0 / 6e2);
-
-struct StepArgs {
-  VmasWorldConfig cfg;
-  VmasPlanTables tb;
-  VmasState st;
-  uint32_t* mask;      // [mask_words + 1]; last word counts blocks that have consumed the mask
-  int use_mask;
-  int mask_words;
-  int first_substep;
-  int n_substeps;
-  const float* ent_params = nullptr;  // [B, E, VMAS_EP_COLS] per-env mass / friction of flagged entities, or null
-};
-
-// an entity's per-env parameter (VMAS_F_*_ENV flag `bit`, column `col` of ent_params) or its scalar column
-DEVI float ent_param(const StepArgs& a, int flg, int bit, long env, int e, int col, const float* ef, int ef_col) {
-  return ((flg & bit) && a.ent_params) ? a.ent_params[((size_t)env * a.cfg.n_entities + e) * VMAS_EP_COLS + col]
-                                       : __ldg(ef + ef_col);
-}
-// moment of inertia: per env from the env's mass (VMAS_F_MASS_ENV), else the scalar column
-DEVI float ent_inertia(const StepArgs& a, int flg, float mass, const float* ef) {
-  return ((flg & VMAS_F_MASS_ENV) && a.ent_params)
-             ? (__ldg(ef + VMAS_EF_INERTIA_K0) * mass) * __ldg(ef + VMAS_EF_INERTIA_K1)
-             : __ldg(ef + VMAS_EF_INERTIA);
-}
-
-// ---------------------------------------------------------------------------------------------
-// per-entity geometry cached in shared memory for the work-item phase
-// ---------------------------------------------------------------------------------------------
-// PITCH = distance (in floats) between consecutive entities of one env: 1 when a group of lanes
-// owns an env (entity-major slice per env), blockDim when one thread owns an env (the thread index
-// is the fastest-varying dimension, so a warp reads 32 consecutive words: no bank conflicts).
-template <int PITCH>
-struct EnvShared {
-  float *px, *py, *rot, *c, *s, *c2, *s2;  // per-entity geometry of this env
-  float *rfx, *rfy, *rta, *rtb;            // per-item results (lane-per-entity kernel only)
-  int pitch;                               // runtime pitch when PITCH == 0
-  DEVI int at(int e) const { return PITCH ? e * PITCH : e * pitch; }
-};
-
-template <int PITCH>
-DEVI V2 ent_pos(const EnvShared<PITCH>& sh, int e) { return mk(sh.px[sh.at(e)], sh.py[sh.at(e)]); }
-
-template <int PITCH>
-DEVI Seg ent_seg(const EnvShared<PITCH>& sh, int e, float length) {
-  return mkseg(ent_pos(sh, e), sh.c[sh.at(e)], sh.s[sh.at(e)], length / 2.f);
-}
-
-template <int PITCH>
-DEVI BoxG ent_box(const EnvShared<PITCH>& sh, int e, float length, float width) {
-  BoxG b;
-  b.p = ent_pos(sh, e);
-  b.c = sh.c[sh.at(e)];
-  b.s = sh.s[sh.at(e)];
-  b.c2 = sh.c2[sh.at(e)];
-  b.s2 = sh.s2[sh.at(e)];
-  b.half_l = length / 2.f;
-  b.half_w = width / 2.f;
-  return b;
-}
-
-// Conservative rejection used before the narrow phase.  A contact force is non-zero only while the
-// two shapes are within their contact threshold of each other; when even the bounding regions are
-// farther apart than that threshold plus FAR_MARGIN (>> any fp32 rounding of these coordinates)
-// the reference's result is an exact 0, which is what skipping produces.
-constexpr float FAR_MARGIN = 1e-3f;
-DEVI bool far_apart(V2 a, V2 b, float reach) {
-  V2 d = a - b;
-  float lim = reach + FAR_MARGIN;
-  return d.x * d.x + d.y * d.y > lim * lim;
-}
-
-// One work item -> (force on a, torque on a, torque on b); the force on b is the negative.
-template <int PITCH>
-DEVI void eval_item(const StepArgs& a, const EnvShared<PITCH>& sh, int item, long env, float* out_fx,
-                    float* out_fy, float* out_ta, float* out_tb) {
-  const int4 ii = __ldg(reinterpret_cast<const int4*>(a.tb.item_i32) + item);
-  const int kind = ii.x, ea = ii.y, eb = ii.z, flags = ii.w & 0xff;
-  const float* f32 = a.tb.item_f32 + (size_t)item * VMAS_IF_COLS;
-  const float dmin_base = __ldg(f32 + VMAS_IF_DMIN_BASE);
-  const float* pa_f = a.tb.ent_f32 + (size_t)ea * VMAS_EF_COLS;
-  const float* pb_f = a.tb.ent_f32 + (size_t)eb * VMAS_EF_COLS;
-  const float cf = a.cfg.collision_force, km = a.cfg.contact_margin;
-  V2 f = mk(0.f, 0.f);
-  float ta = 0.f, tb = 0.f;
-
-  switch (kind) {
-    case VMAS_K_JOINT: {  // ref core.py:2201-2292, joints.py:209-216
-      V2 pa = ent_pos(sh, ea), pb = ent_pos(sh, eb);
-      V2 da = mk(__ldg(f32 + VMAS_IF_AX), __ldg(f32 + VMAS_IF_AY));
-      V2 db = mk(__ldg(f32 + VMAS_IF_BX), __ldg(f32 + VMAS_IF_BY));
-      V2 qa = pa + rot2(da, sh.c[sh.at(ea)], sh.s[sh.at(ea)]);
-      V2 qb = pb + rot2(db, sh.c[sh.at(eb)], sh.s[sh.at(eb)]);
-      float dist = __ldg(f32 + VMAS_IF_DIST);
-      V2 f_attr = constraint_force(qa, qb, dist, a.cfg.joint_force, km, true);
-      V2 f_rep = constraint_force(qa, qb, dist, a.cfg.joint_force, km, false);
-      f = f_attr + f_rep;
-      V2 fb = neg(f_attr) + neg(f_rep);
-      ta = cross2(qa - pa, f);
-      tb = cross2(qb - pb, fb);
-      if (!(flags & VMAS_IFLAG_JOINT_ROTATE)) {  // ref core.py:2841-2858
-        float jr = (flags & VMAS_IFLAG_JOINT_ROT_PER_ENV)
-                       ? a.tb.joint_rot[(size_t)env * a.cfg.n_joints + item]
-                       : __ldg(f32 + VMAS_IF_FIXED_ROT);
-        float ra = sh.rot[sh.at(ea)], rb = sh.rot[sh.at(eb)];
-        float delta = ra - (rb + jr);
-        float mag = sqrtf(delta * delta);
-        float t = (a.cfg.torque_constraint_force * sgnf(delta)) * (expf(mag) - 1.f);
-        if (mag < 1e-9f) t = 0.f;
-        ta = ta + (-t);
-        tb = tb + t;
-      }
-      break;
-    }
-    case VMAS_K_SS: {  // ref core.py:2294-2339
-      f = constraint_force(ent_pos(sh, ea), ent_pos(sh, eb), dmin_base, cf, km, false);
-      break;
-    }
-    case VMAS_K_LS: {  // a = line, b = sphere; ref core.py:2341-2392
-      Seg l = ent_seg(sh, ea, __ldg(pa_f + VMAS_EF_D0));
-      V2 ps = ent_pos(sh, eb);
-      if (far_apart(l.p, ps, l.half + dmin_base)) break;
-      V2 cp = closest_point_seg(l, ps);
-      V2 f_sphere = constraint_force(ps, cp, dmin_base, cf, km, false);
-      f = neg(f_sphere);  // force on the line
-      ta = cross2(cp - l.p, f);
-      break;
-    }
-    case VMAS_K_LL: {  // ref core.py:2394-2457
-      Seg l1 = ent_seg(sh, ea, __ldg(pa_f + VMAS_EF_D0));
-      Seg l2 = ent_seg(sh, eb, __ldg(pb_f + VMAS_EF_D0));
-      if (far_apart(l1.p, l2.p, l1.half + l2.half + dmin_base)) break;
-      Pair c = closest_seg_seg(l1, l2);
-      f = constraint_force(c.a, c.b, dmin_base, cf, km, false);
-      ta = cross2(c.a - l1.p, f);
-      tb = cross2(c.b - l2.p, neg(f));
-      break;
-    }
-    case VMAS_K_BS: {  // a = box, b = sphere; ref core.py:2459-2552
-      BoxG bx = ent_box(sh, ea, __ldg(pa_f + VMAS_EF_D0), __ldg(pa_f + VMAS_EF_D1));
-      const bool hollow = __ldg(a.tb.ent_i32 + ea * 4 + 1) & VMAS_F_HOLLOW;
-      V2 ps = ent_pos(sh, eb);
-      {  // sphere centre outside the box inflated by r + LINE_MIN_DIST (+ margin): force is exactly 0
-        V2 d = ps - bx.p;
-        float lx = d.x * bx.c + d.y * bx.s, ly = d.y * bx.c - d.x * bx.s;
-        if (fabsf(lx) > bx.half_l + dmin_base + FAR_MARGIN || fabsf(ly) > bx.half_w + dmin_base + FAR_MARGIN) break;
-      }
-      V2 cp = closest_point_box(bx, ps);
-      V2 inner = cp;
-      float d = 0.f;
-      if (!hollow) inner = inner_point_box(ps, cp, bx.p, &d);
-      V2 f_sphere = constraint_force(ps, inner, dmin_base + d, cf, km, false);
-      f = neg(f_sphere);  // force on the box
-      ta = cross2(cp - bx.p, f);
-      break;
-    }
-    case VMAS_K_BL: {  // a = box, b = line; ref core.py:2554-2653
-      BoxG bx = ent_box(sh, ea, __ldg(pa_f + VMAS_EF_D0), __ldg(pa_f + VMAS_EF_D1));
-      const bool hollow = __ldg(a.tb.ent_i32 + ea * 4 + 1) & VMAS_F_HOLLOW;
-      Seg l = ent_seg(sh, eb, __ldg(pb_f + VMAS_EF_D0));
-      {  // segment entirely outside the box inflated by LINE_MIN_DIST (+ margin): force is exactly 0
-        V2 d = l.p - bx.p;
-        float lx = d.x * bx.c + d.y * bx.s, ly = d.y * bx.c - d.x * bx.s;
-        float ex = l.half * fabsf(l.c * bx.c + l.s * bx.s), ey = l.half * fabsf(l.s * bx.c - l.c * bx.s);
-        if (fabsf(lx) - ex > bx.half_l + dmin_base + FAR_MARGIN || fabsf(ly) - ey > bx.half_w + dmin_base + FAR_MARGIN)
-          break;
-      }
-      Pair c = closest_box_seg(bx, l);
-      V2 inner = c.a;
-      float d = 0.f;
-      if (!hollow) inner = inner_point_box(c.b, c.a, bx.p, &d);
-      f = constraint_force(inner, c.b, dmin_base + d, cf, km, false);
-      ta = cross2(c.a - bx.p, f);
-      tb = cross2(c.b - l.p, neg(f));
-      break;
-    }
-    case VMAS_K_BB: {  // ref core.py:2655-2786
-      BoxG b1 = ent_box(sh, ea, __ldg(pa_f + VMAS_EF_D0), __ldg(pa_f + VMAS_EF_D1));
-      BoxG b2 = ent_box(sh, eb, __ldg(pb_f + VMAS_EF_D0), __ldg(pb_f + VMAS_EF_D1));
-      const bool hollow1 = __ldg(a.tb.ent_i32 + ea * 4 + 1) & VMAS_F_HOLLOW;
-      const bool hollow2 = __ldg(a.tb.ent_i32 + eb * 4 + 1) & VMAS_F_HOLLOW;
-      if (far_apart(b1.p, b2.p, __ldg(pa_f + VMAS_EF_CIRC_R) + __ldg(pb_f + VMAS_EF_CIRC_R) + dmin_base)) break;
-      Pair c = closest_box_box(b1, b2);
-      V2 in1 = c.a, in2 = c.b;
-      float d1 = 0.f, d2 = 0.f;
-      if (!hollow1) in1 = inner_point_box(c.b, c.a, b1.p, &d1);
-      if (!hollow2) in2 = inner_point_box(c.a, c.b, b2.p, &d2);
-      f = constraint_force(in1, in2, (d1 + d2) + dmin_base, cf, km, false);
-      ta = cross2(c.a - b1.p, f);
-      tb = cross2(c.b - b2.p, neg(f));
-      break;
-    }
-    default:
-      break;
-  }
-  *out_fx = f.x;
-  *out_fy = f.y;
-  *out_ta = ta;
-  *out_tb = tb;
-}
 
 // ---------------------------------------------------------------------------------------------
 // the fused substep kernel
@@ -527,8 +328,6 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
 // reference's order, and no intra-env synchronisation is needed.  The env's state lives in shared
 // memory as [field][entity][thread] so a warp always touches 32 consecutive words.
 // ---------------------------------------------------------------------------------------------
-enum { T_PX = 0, T_PY, T_ROT, T_C, T_S, T_C2, T_S2, T_VX, T_VY, T_W, T_FX, T_FY, T_TQ, T_NF };
-
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK) step_tpe_kernel(const StepArgs a) {
   extern __shared__ float smem[];
@@ -566,205 +365,80 @@ __global__ void __launch_bounds__(BLOCK) step_tpe_kernel(const StepArgs a) {
   sh.rfx = sh.rfy = sh.rta = sh.rtb = nullptr;
 
   const size_t ebase = (size_t)env * E, abase = (size_t)env * A;
-  const float2* gpos = reinterpret_cast<const float2*>(a.st.pos) + ebase;
-  const float2* gvel = reinterpret_cast<const float2*>(a.st.vel) + ebase;
-
-  // ---- load the env's slab ------------------------------------------------------------------
-  for (int e = 0; e < E; ++e) {
-    const int flg = __ldg(a.tb.ent_i32 + e * 4 + 1);
-    const float2 p = gpos[e];
-    TF(T_PX, e) = p.x;
-    TF(T_PY, e) = p.y;
-    TF(T_ROT, e) = a.st.rot[ebase + e];
-    float2 v = make_float2(0.f, 0.f);
-    if (flg & VMAS_F_MOVABLE) v = gvel[e];
-    TF(T_VX, e) = v.x;
-    TF(T_VY, e) = v.y;
-    TF(T_W, e) = (flg & VMAS_F_ROTATABLE) ? a.st.ang_vel[ebase + e] : 0.f;
-  }
+  for (int e = 0; e < E; ++e) entity_load<BLOCK>(a, col, E, e, ebase);
 
   const float sub_dt = a.cfg.sub_dt;
   for (int sub = a.first_substep; sub < a.first_substep + a.n_substeps; ++sub) {
-    // ---- phase A: trig cache + per-entity forces (ref core.py:1995-2004) -------------------
-    for (int e = 0; e < E; ++e) {
-      const int flg = __ldg(a.tb.ent_i32 + e * 4 + 1);
-      const float* ef = a.tb.ent_f32 + (size_t)e * VMAS_EF_COLS;
-      if (flg & VMAS_F_TRIG) {
-        const float r = TF(T_ROT, e);
-        float sn, cs;
-        sincosf(r, &sn, &cs);
-        TF(T_C, e) = cs;
-        TF(T_S, e) = sn;
-        if (__ldg(a.tb.ent_i32 + e * 4) == VMAS_SHAPE_BOX) {
-          sincosf(r + HALF_PI_F, &sn, &cs);
-          TF(T_C2, e) = cs;
-          TF(T_S2, e) = sn;
-        }
-      }
-      float Fx = 0.f, Fy = 0.f, T = 0.f;
-      const float mass = ent_param(a, flg, VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS);
-      if (flg & VMAS_F_AGENT) {  // ref core.py:2018-2041
-        const int ai = __ldg(a.tb.ent_i32 + e * 4 + 2);
-        if (flg & VMAS_F_MOVABLE) {
-          float2 af = reinterpret_cast<const float2*>(a.st.force)[abase + ai];
-          if (flg & (VMAS_F_MAX_F | VMAS_F_F_RANGE)) {
-            if (flg & VMAS_F_MAX_F) {
-              const float mx = __ldg(ef + VMAS_EF_MAX_F);
-              const float n = norm2(af.x, af.y);
-              if (n > mx) {
-                af.x = (af.x / n) * mx;
-                af.y = (af.y / n) * mx;
-              }
-            }
-            if (flg & VMAS_F_F_RANGE) {
-              const float r = __ldg(ef + VMAS_EF_F_RANGE);
-              af.x = fminf(fmaxf(af.x, -r), r);
-              af.y = fminf(fmaxf(af.y, -r), r);
-            }
-            reinterpret_cast<float2*>(a.st.force)[abase + ai] = af;
-          }
-          Fx = Fx + af.x;
-          Fy = Fy + af.y;
-        }
-        if (flg & VMAS_F_ROTATABLE) {
-          float tq = a.st.torque[abase + ai];
-          if (flg & (VMAS_F_MAX_T | VMAS_F_T_RANGE)) {
-            if (flg & VMAS_F_MAX_T) {
-              const float mx = __ldg(ef + VMAS_EF_MAX_T);
-              const float n = sqrtf(tq * tq);
-              if (n > mx) tq = (tq / n) * mx;
-            }
-            if (flg & VMAS_F_T_RANGE) {
-              const float r = __ldg(ef + VMAS_EF_T_RANGE);
-              tq = fminf(fmaxf(tq, -r), r);
-            }
-            a.st.torque[abase + ai] = tq;
-          }
-          T = T + tq;
-        }
-      }
-      if (flg & VMAS_F_LIN_FRIC) {  // ref core.py:2054-2088
-        const float vx = TF(T_VX, e), vy = TF(T_VY, e);
-        const float speed = norm2(vx, vy);
-        if (speed != 0.f) {
-          const float cap = ent_param(a, flg, VMAS_F_LIN_FRIC_ENV, env, e, VMAS_EP_LIN_FRIC, ef, VMAS_EF_LIN_FRIC) * mass;
-          Fx = Fx + (-(vx / speed)) * fminf(cap, (fabsf(vx) / sub_dt) * mass);
-          Fy = Fy + (-(vy / speed)) * fminf(cap, (fabsf(vy) / sub_dt) * mass);
-        }
-      }
-      if (flg & VMAS_F_ANG_FRIC) {  // ref core.py:2089-2102
-        const float w = TF(T_W, e);
-        const float speed = sqrtf(w * w);
-        if (speed != 0.f) {
-          const float inertia = ent_inertia(a, flg, mass, ef);
-          const float cap = ent_param(a, flg, VMAS_F_ANG_FRIC_ENV, env, e, VMAS_EP_ANG_FRIC, ef, VMAS_EF_ANG_FRIC) * inertia;
-          T = T + (-(w / speed)) * fminf(cap, (fabsf(w) / sub_dt) * inertia);
-        }
-      }
-      if (flg & VMAS_F_MOVABLE) {  // ref core.py:2043-2052
-        if (a.cfg.has_world_gravity) {
-          Fx = Fx + mass * a.cfg.gravity_x;
-          Fy = Fy + mass * a.cfg.gravity_y;
-        }
-        if (flg & VMAS_F_GRAVITY) {
-          Fx = Fx + mass * __ldg(ef + VMAS_EF_GRAV_X);
-          Fy = Fy + mass * __ldg(ef + VMAS_EF_GRAV_Y);
-        }
-        if (flg & VMAS_F_GRAVITY_ENV) {
-          const float2 g = reinterpret_cast<const float2*>(a.tb.ent_gravity)[ebase + e];
-          Fx = Fx + mass * g.x;
-          Fy = Fy + mass * g.y;
-        }
-      }
-      TF(T_FX, e) = Fx;
-      TF(T_FY, e) = Fy;
-      TF(T_TQ, e) = T;
-    }
-
+    // ---- phase A: trig cache + per-entity forces --------------------------------------------
+    for (int e = 0; e < E; ++e) entity_forces<BLOCK>(a, col, E, e, env, ebase, abase, sub_dt);
     // ---- phase B: joints and contacts in the reference's accumulation order -----------------
-    for (int item = 0; item < NI; ++item) {
-      const int4 ii = __ldg(reinterpret_cast<const int4*>(a.tb.item_i32) + item);
-      if (a.use_mask) {
-        const int mbit = (ii.w >> 8) - 1;
-        if (mbit >= 0 && !((s_mask[mbit >> 5] >> (mbit & 31)) & 1u)) continue;
-      }
-      float fx, fy, ta, tb;
-      eval_item(a, sh, item, env, &fx, &fy, &ta, &tb);
-      const int fa = __ldg(a.tb.ent_i32 + ii.y * 4 + 1), fb = __ldg(a.tb.ent_i32 + ii.z * 4 + 1);
-      if (fa & VMAS_F_MOVABLE) {
-        TF(T_FX, ii.y) = TF(T_FX, ii.y) + fx;
-        TF(T_FY, ii.y) = TF(T_FY, ii.y) + fy;
-      }
-      if (fa & VMAS_F_ROTATABLE) TF(T_TQ, ii.y) = TF(T_TQ, ii.y) + ta;
-      if (fb & VMAS_F_MOVABLE) {
-        TF(T_FX, ii.z) = TF(T_FX, ii.z) + (-fx);
-        TF(T_FY, ii.z) = TF(T_FY, ii.z) + (-fy);
-      }
-      if (fb & VMAS_F_ROTATABLE) TF(T_TQ, ii.z) = TF(T_TQ, ii.z) + tb;
-    }
-
-    // ---- phase C: semi-implicit Euler (ref core.py:2862-2908) ------------------------------
-    for (int e = 0; e < E; ++e) {
-      const int flg = __ldg(a.tb.ent_i32 + e * 4 + 1);
-      if (!(flg & (VMAS_F_MOVABLE | VMAS_F_ROTATABLE))) continue;
-      const float* ef = a.tb.ent_f32 + (size_t)e * VMAS_EF_COLS;
-      const float drag_mult = __ldg(ef + VMAS_EF_DRAG_MULT);
-      if (flg & VMAS_F_MOVABLE) {
-        const float mass = ent_param(a, flg, VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS);
-        float vx = TF(T_VX, e), vy = TF(T_VY, e);
-        if (sub == 0) {
-          vx = vx * drag_mult;
-          vy = vy * drag_mult;
-        }
-        vx = vx + div_pos(TF(T_FX, e), mass) * sub_dt;
-        vy = vy + div_pos(TF(T_FY, e), mass) * sub_dt;
-        if (flg & VMAS_F_MAX_SPEED) {
-          const float mx = __ldg(ef + VMAS_EF_MAX_SPEED);
-          const float n = norm2(vx, vy);
-          if (n > mx) {
-            vx = (vx / n) * mx;
-            vy = (vy / n) * mx;
-          }
-        }
-        if (flg & VMAS_F_V_RANGE) {
-          const float r = __ldg(ef + VMAS_EF_V_RANGE);
-          vx = fminf(fmaxf(vx, -r), r);
-          vy = fminf(fmaxf(vy, -r), r);
-        }
-        float px = TF(T_PX, e) + vx * sub_dt;
-        float py = TF(T_PY, e) + vy * sub_dt;
-        if (a.cfg.has_x_semidim) px = fminf(fmaxf(px, -a.cfg.x_semidim), a.cfg.x_semidim);
-        if (a.cfg.has_y_semidim) py = fminf(fmaxf(py, -a.cfg.y_semidim), a.cfg.y_semidim);
-        TF(T_VX, e) = vx;
-        TF(T_VY, e) = vy;
-        TF(T_PX, e) = px;
-        TF(T_PY, e) = py;
-      }
-      if (flg & VMAS_F_ROTATABLE) {
-        const float inertia =
-            ent_inertia(a, flg, ent_param(a, flg, VMAS_F_MASS_ENV, env, e, VMAS_EP_MASS, ef, VMAS_EF_MASS), ef);
-        float w = TF(T_W, e);
-        if (sub == 0) w = w * drag_mult;
-        w = w + div_pos(TF(T_TQ, e), inertia) * sub_dt;
-        TF(T_W, e) = w;
-        TF(T_ROT, e) = TF(T_ROT, e) + w * sub_dt;
-      }
-    }
+    for (int item = 0; item < NI; ++item) item_accumulate(a, sh, col, E, item, env, s_mask);
+    // ---- phase C: semi-implicit Euler ---------------------------------------------------------
+    for (int e = 0; e < E; ++e) entity_integrate<BLOCK>(a, col, E, e, env, sub, sub_dt);
   }
-
-  // ---- write-back: only what can have changed --------------------------------------------------
-  for (int e = 0; e < E; ++e) {
-    const int flg = __ldg(a.tb.ent_i32 + e * 4 + 1);
-    if (flg & VMAS_F_MOVABLE) {
-      reinterpret_cast<float2*>(a.st.pos)[ebase + e] = make_float2(TF(T_PX, e), TF(T_PY, e));
-      reinterpret_cast<float2*>(a.st.vel)[ebase + e] = make_float2(TF(T_VX, e), TF(T_VY, e));
-    }
-    if (flg & VMAS_F_ROTATABLE) {
-      a.st.rot[ebase + e] = TF(T_ROT, e);
-      a.st.ang_vel[ebase + e] = TF(T_W, e);
-    }
-  }
+  for (int e = 0; e < E; ++e) entity_store<BLOCK>(a, col, E, e, ebase);
 #undef TF
+}
+
+// ---------------------------------------------------------------------------------------------
+// block-per-env substep kernel (worlds whose thread-per-env layout does not fit in shared memory)
+//
+// One block owns one env; thread t owns entities t, t + BLOCK, ...  The env's state lives in shared
+// memory as [field][entity] (52 B per entity), the broad-phase mask words behind it.  Phase B walks
+// each entity's incidence list: every work item is evaluated twice, once by each endpoint's owner,
+// which keeps its own side.  That costs one extra evaluation per item and saves the result staging
+// and the atomics; each entity's sums have the operands and the order of step_tpe_kernel's, so the
+// two kernels produce the same bits.
+// ---------------------------------------------------------------------------------------------
+constexpr int STEP_BLOCK_THREADS = 128;
+
+__global__ void __launch_bounds__(STEP_BLOCK_THREADS) step_block_kernel(const StepArgs a) {
+  constexpr int BLOCK = STEP_BLOCK_THREADS;
+  extern __shared__ float smem[];
+  const int E = a.cfg.n_entities, A = a.cfg.n_agents;
+  const int tid = threadIdx.x;
+  const long env = blockIdx.x;  // grid = batch_dim: every block owns a live env
+  float* const col = smem;
+  uint32_t* s_mask = reinterpret_cast<uint32_t*>(smem + (size_t)T_NF * E);
+
+  if (a.use_mask) {
+    for (int w = tid; w < a.mask_words; w += BLOCK) s_mask[w] = a.mask[w];
+    __syncthreads();
+    if (tid == 0) {  // the last block to have copied the mask clears it for the next pass
+      __threadfence();
+      unsigned done = atomicAdd(&a.mask[a.mask_words], 1u);
+      if (done == gridDim.x - 1) {
+        for (int w = 0; w < a.mask_words; ++w) a.mask[w] = 0u;
+        a.mask[a.mask_words] = 0u;
+      }
+    }
+  }
+
+  EnvShared<1> sh;
+  sh.pitch = 1;
+  sh.px = smem + (size_t)T_PX * E;
+  sh.py = smem + (size_t)T_PY * E;
+  sh.rot = smem + (size_t)T_ROT * E;
+  sh.c = smem + (size_t)T_C * E;
+  sh.s = smem + (size_t)T_S * E;
+  sh.c2 = smem + (size_t)T_C2 * E;
+  sh.s2 = smem + (size_t)T_S2 * E;
+  sh.rfx = sh.rfy = sh.rta = sh.rtb = nullptr;
+
+  const size_t ebase = (size_t)env * E, abase = (size_t)env * A;
+  for (int e = tid; e < E; e += BLOCK) entity_load<1>(a, col, E, e, ebase);
+  __syncthreads();
+
+  const float sub_dt = a.cfg.sub_dt;
+  for (int sub = a.first_substep; sub < a.first_substep + a.n_substeps; ++sub) {
+    for (int e = tid; e < E; e += BLOCK) entity_forces<1>(a, col, E, e, env, ebase, abase, sub_dt);
+    __syncthreads();  // every entity's trig cache is published
+    for (int e = tid; e < E; e += BLOCK) entity_accumulate(a, sh, col, E, e, env, s_mask);
+    __syncthreads();  // nobody reads positions any more
+    for (int e = tid; e < E; e += BLOCK) entity_integrate<1>(a, col, E, e, env, sub, sub_dt);
+    __syncthreads();  // the next substep reads the new positions
+  }
+  for (int e = tid; e < E; e += BLOCK) entity_store<1>(a, col, E, e, ebase);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1318,6 +992,19 @@ __global__ void __launch_bounds__(256) gather_observations_kernel(const ObsArgs 
   gather_observations_body<VEC>(a, tile_envs, blockIdx.y);
 }
 
+// The observation launches stage a tile of envs' slab rows in shared memory: a multiple of 4 envs (keeps every
+// field's tile 16-byte aligned) whose state fits 32 KB.  Past ~500 entities even 4 envs need more than the
+// default 48 KB; the launch then opts into more dynamic shared memory, up to VMAS_BLOCK_MAX_ENTITIES.
+static int obs_tile(int n_entities, int* tile_out, size_t* smem_out) {
+  if (n_entities > VMAS_BLOCK_MAX_ENTITIES) return fail("observation rows of worlds with more than 1024 entities%s");
+  const size_t per_env = 6u * (size_t)n_entities * sizeof(float);
+  int tile = 128;
+  while (tile > 4 && tile * per_env + 64 > 32 * 1024) tile /= 2;
+  *tile_out = tile;
+  *smem_out = tile * per_env + 64;
+  return 0;
+}
+
 // ---------------------------------------------------------------------------------------------
 // post-step program: the scenario's reward / done glue as ONE launch together with the observation
 // gather.  A scenario's callbacks are a handful of distance / overlap queries, the distance-shaping
@@ -1522,6 +1209,28 @@ static int dispatch_tpe(const StepArgs& args, cudaStream_t stream) {
   return r;
 }
 
+static int launch_block(const StepArgs& args, cudaStream_t stream) {
+  if (args.cfg.n_entities > VMAS_BLOCK_MAX_ENTITIES)
+    return fail("world too large: the block-per-env step takes at most 1024 entities%s");
+  int device = 0;
+  CUDA_OK(cudaGetDevice(&device));
+  static int max_optin[64] = {0};
+  if (device < 64 && max_optin[device] == 0)
+    CUDA_OK(cudaDeviceGetAttribute(&max_optin[device], cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+  const size_t limit = device < 64 ? (size_t)max_optin[device] : 48 * 1024;
+  const size_t smem = (size_t)T_NF * args.cfg.n_entities * sizeof(float) +
+                      (size_t)(args.use_mask ? args.mask_words : 0) * sizeof(uint32_t);
+  if (smem > limit) return fail("world too large: an env's state does not fit in shared memory%s");
+  static size_t configured[64] = {0};
+  if (smem > 48 * 1024 && (device >= 64 || configured[device] < smem)) {
+    CUDA_OK(cudaFuncSetAttribute(step_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
+    if (device < 64) configured[device] = limit;
+  }
+  step_block_kernel<<<(unsigned)args.cfg.batch_dim, STEP_BLOCK_THREADS, smem, stream>>>(args);
+  CUDA_OK(cudaGetLastError());
+  return 1;
+}
+
 // specialisations compiled at run time (vmas_b200_register_specialization): indices kNumSpecs, ...
 static SpecEntry g_dyn_specs[VMAS_MAX_RUNTIME_SPECS];
 static int g_num_dyn_specs = 0;
@@ -1595,6 +1304,7 @@ static int dispatch_step(const StepArgs& args, cudaStream_t stream) {
     return dispatch_spec(args, stream);
   }
   if (args.tb.group == 1) return dispatch_tpe(args, stream);
+  if (args.tb.group == VMAS_GROUP_BLOCK) return launch_block(args, stream);
   const int G = args.tb.group, EPL = args.tb.ents_per_lane;
   if (G == 8 && EPL == 1) return launch_step<8, 1>(args, stream);
   if (G == 16 && EPL == 1) return launch_step<16, 1>(args, stream);
@@ -2078,20 +1788,13 @@ int vmas_b200_gather_observations_buffers(const VmasWorldConfig* cfg, const Vmas
   if (groups > 256) return fail("observation rows wider than 1024 columns are not supported%s");
   const unsigned bx = (unsigned)groups, by = 256 / bx;
   const dim3 block(bx, by);
-  // tile: a multiple of 4 envs (keeps every field's tile 16-byte aligned) whose state fits 32 KB
-  const size_t per_env = 6u * (size_t)cfg->n_entities * sizeof(float);
-  int tile = 128;
-  while (tile > 4 && tile * per_env + 64 > 32 * 1024) tile /= 2;
-  if (tile * per_env + 64 > 48 * 1024) return fail("worlds with more than ~500 entities are not supported here%s");
-  const size_t smem = tile * per_env + 64;
+  int tile = 0;
+  size_t smem = 0;
+  if (obs_tile(cfg->n_entities, &tile, &smem) < 0) return -1;
   const dim3 grid((unsigned)((cfg->batch_dim + tile - 1) / tile), (unsigned)n_rows);
-  if (vec == 4) {
-    gather_observations_kernel<4><<<grid, block, smem, stream>>>(a, tile);
-  } else if (vec == 2) {
-    gather_observations_kernel<2><<<grid, block, smem, stream>>>(a, tile);
-  } else {
-    gather_observations_kernel<1><<<grid, block, smem, stream>>>(a, tile);
-  }
+  auto kern = vec == 4 ? gather_observations_kernel<4> : vec == 2 ? gather_observations_kernel<2> : gather_observations_kernel<1>;
+  if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<grid, block, smem, stream>>>(a, tile);
   CUDA_OK(cudaGetLastError());
   return 1;
 }
@@ -2137,19 +1840,13 @@ int vmas_b200_post_step(const VmasWorldConfig* cfg, const VmasPlanTables* tb, co
   if (groups > 256 || groups < 1) return fail("observation rows wider than 1024 columns are not supported%s");
   const unsigned bx = (unsigned)groups, by = 256 / bx;
   const dim3 block(bx, by);
-  const size_t per_env = 6u * (size_t)cfg->n_entities * sizeof(float);
-  int tile = 128;
-  while (tile > 4 && tile * per_env + 64 > 32 * 1024) tile /= 2;
-  if (tile * per_env + 64 > 48 * 1024) return fail("worlds with more than ~500 entities are not supported here%s");
-  const size_t smem = tile * per_env + 64;
+  int tile = 0;
+  size_t smem = 0;
+  if (obs_tile(cfg->n_entities, &tile, &smem) < 0) return -1;
   const dim3 grid((unsigned)((cfg->batch_dim + tile - 1) / tile), (unsigned)(oa.rows + (has_prog ? 1 : 0)));
-  if (vec == 4) {
-    post_step_kernel<4><<<grid, block, smem, stream>>>(oa, tile, pa);
-  } else if (vec == 2) {
-    post_step_kernel<2><<<grid, block, smem, stream>>>(oa, tile, pa);
-  } else {
-    post_step_kernel<1><<<grid, block, smem, stream>>>(oa, tile, pa);
-  }
+  auto kern = vec == 4 ? post_step_kernel<4> : vec == 2 ? post_step_kernel<2> : post_step_kernel<1>;
+  if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<grid, block, smem, stream>>>(oa, tile, pa);
   CUDA_OK(cudaGetLastError());
   return 1;
 }
