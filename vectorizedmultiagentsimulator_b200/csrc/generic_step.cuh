@@ -263,8 +263,8 @@ DEVI void entity_forces(const StepArgs& a, float* col, int E, int e, long env, s
         }
         if (flg & VMAS_F_F_RANGE) {
           const float r = __ldg(ef + VMAS_EF_F_RANGE);
-          af.x = fminf(fmaxf(af.x, -r), r);
-          af.y = fminf(fmaxf(af.y, -r), r);
+          af.x = clampf(af.x, -r, r);
+          af.y = clampf(af.y, -r, r);
         }
         reinterpret_cast<float2*>(a.st.force)[abase + ai] = af;
       }
@@ -276,12 +276,12 @@ DEVI void entity_forces(const StepArgs& a, float* col, int E, int e, long env, s
       if (flg & (VMAS_F_MAX_T | VMAS_F_T_RANGE)) {
         if (flg & VMAS_F_MAX_T) {
           const float mx = __ldg(ef + VMAS_EF_MAX_T);
-          const float n = sqrtf(tq * tq);
+          const float n = fabsf(tq);  // vector_norm of one element
           if (n > mx) tq = (tq / n) * mx;
         }
         if (flg & VMAS_F_T_RANGE) {
           const float r = __ldg(ef + VMAS_EF_T_RANGE);
-          tq = fminf(fmaxf(tq, -r), r);
+          tq = clampf(tq, -r, r);
         }
         a.st.torque[abase + ai] = tq;
       }
@@ -299,7 +299,7 @@ DEVI void entity_forces(const StepArgs& a, float* col, int E, int e, long env, s
   }
   if (flg & VMAS_F_ANG_FRIC) {  // ref core.py:2089-2102
     const float w = GS_F(T_W, e);
-    const float speed = sqrtf(w * w);
+    const float speed = fabsf(w);  // vector_norm of one element
     if (speed != 0.f) {
       const float inertia = ent_inertia(a, flg, mass, ef);
       const float cap = ent_param(a, flg, VMAS_F_ANG_FRIC_ENV, env, e, VMAS_EP_ANG_FRIC, ef, VMAS_EF_ANG_FRIC) * inertia;
@@ -422,13 +422,13 @@ DEVI void entity_integrate(const StepArgs& a, float* col, int E, int e, long env
     }
     if (flg & VMAS_F_V_RANGE) {
       const float r = __ldg(ef + VMAS_EF_V_RANGE);
-      vx = fminf(fmaxf(vx, -r), r);
-      vy = fminf(fmaxf(vy, -r), r);
+      vx = clampf(vx, -r, r);
+      vy = clampf(vy, -r, r);
     }
     float px = GS_F(T_PX, e) + vx * sub_dt;
     float py = GS_F(T_PY, e) + vy * sub_dt;
-    if (a.cfg.has_x_semidim) px = fminf(fmaxf(px, -a.cfg.x_semidim), a.cfg.x_semidim);
-    if (a.cfg.has_y_semidim) py = fminf(fmaxf(py, -a.cfg.y_semidim), a.cfg.y_semidim);
+    if (a.cfg.has_x_semidim) px = clampf(px, -a.cfg.x_semidim, a.cfg.x_semidim);
+    if (a.cfg.has_y_semidim) py = clampf(py, -a.cfg.y_semidim, a.cfg.y_semidim);
     GS_F(T_VX, e) = vx;
     GS_F(T_VY, e) = vy;
     GS_F(T_PX, e) = px;

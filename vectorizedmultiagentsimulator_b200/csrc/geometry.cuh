@@ -41,6 +41,22 @@ DEVI float div_pos(float a, float b) {
   const float q = (zero ? 1.f : a) / b;
   return zero ? a : q;
 }
+// torch.clamp(x, lo, hi): a NaN stays NaN, where fminf(fmaxf(x, lo), hi) would return a bound and let a
+// NaN force, velocity or position carry on as finite state.  Any other x gives fminf(fmaxf(x, lo), hi)'s
+// bits, signed zeros included: max.NaN / min.NaN (sm_80+) differ from max / min only in NaN handling.
+// The host build (tests/hostsim) spells out the same order, -0 below +0, rather than trust libm's.
+DEVI float clampf(float x, float lo, float hi) {
+#ifdef __CUDA_ARCH__
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(x), "f"(lo));
+  asm("min.NaN.f32 %0, %0, %1;" : "+f"(r) : "f"(hi));
+  return r;
+#else
+  if (x != x) return x;
+  const float m = (x > lo || (x == lo && !signbit(x))) ? x : lo;
+  return (m < hi || (m == hi && signbit(m))) ? m : hi;
+#endif
+}
 // rotate `v` by the angle whose (cos, sin) is (c, s)  (ref utils.py:176-191)
 DEVI V2 rot2(V2 v, float c, float s) { return mk(v.x * c - v.y * s, v.x * s + v.y * c); }
 

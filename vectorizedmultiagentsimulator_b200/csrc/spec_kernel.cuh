@@ -637,18 +637,18 @@ DEVI void spec_entity_forces(EnvRegs<E>& r, float (&afx)[NAX], float (&afy)[NAX]
           }
         }
         if constexpr (en.flags & VMAS_F_F_RANGE) {
-          afx[ai] = fminf(fmaxf(afx[ai], -en.f_range), en.f_range);
-          afy[ai] = fminf(fmaxf(afy[ai], -en.f_range), en.f_range);
+          afx[ai] = clampf(afx[ai], -en.f_range, en.f_range);
+          afy[ai] = clampf(afy[ai], -en.f_range, en.f_range);
         }
         Fx = Fx + afx[ai];
         Fy = Fy + afy[ai];
       }
       if constexpr (en.flags & VMAS_F_ROTATABLE) {
         if constexpr (en.flags & VMAS_F_MAX_T) {
-          const float n = sqrtf(atq[ai] * atq[ai]);
+          const float n = fabsf(atq[ai]);  // vector_norm of one element
           if (n > en.max_t) atq[ai] = (atq[ai] / n) * en.max_t;
         }
-        if constexpr (en.flags & VMAS_F_T_RANGE) atq[ai] = fminf(fmaxf(atq[ai], -en.t_range), en.t_range);
+        if constexpr (en.flags & VMAS_F_T_RANGE) atq[ai] = clampf(atq[ai], -en.t_range, en.t_range);
         T = T + atq[ai];
       }
     }
@@ -662,7 +662,7 @@ DEVI void spec_entity_forces(EnvRegs<E>& r, float (&afx)[NAX], float (&afy)[NAX]
       }
     }
     if constexpr (en.flags & VMAS_F_ANG_FRIC) {
-      const float speed = sqrtf(r.w[e] * r.w[e]);
+      const float speed = fabsf(r.w[e]);  // vector_norm of one element
       if (speed != 0.f) {
         const float inertia = spec_inertia<W, e>(pe);
         const float cap = spec_ang_fric<W, e>(pe) * inertia;
@@ -712,13 +712,13 @@ DEVI void spec_integrate(EnvRegs<E>& r, const int sub, const SpecEnvParams<W>* p
         }
       }
       if constexpr (en.flags & VMAS_F_V_RANGE) {
-        r.vx[e] = fminf(fmaxf(r.vx[e], -en.v_range), en.v_range);
-        r.vy[e] = fminf(fmaxf(r.vy[e], -en.v_range), en.v_range);
+        r.vx[e] = clampf(r.vx[e], -en.v_range, en.v_range);
+        r.vy[e] = clampf(r.vy[e], -en.v_range, en.v_range);
       }
       r.px[e] = r.px[e] + r.vx[e] * sub_dt;
       r.py[e] = r.py[e] + r.vy[e] * sub_dt;
-      if constexpr (W::cfg.has_x_semidim) r.px[e] = fminf(fmaxf(r.px[e], -W::cfg.x_semidim), W::cfg.x_semidim);
-      if constexpr (W::cfg.has_y_semidim) r.py[e] = fminf(fmaxf(r.py[e], -W::cfg.y_semidim), W::cfg.y_semidim);
+      if constexpr (W::cfg.has_x_semidim) r.px[e] = clampf(r.px[e], -W::cfg.x_semidim, W::cfg.x_semidim);
+      if constexpr (W::cfg.has_y_semidim) r.py[e] = clampf(r.py[e], -W::cfg.y_semidim, W::cfg.y_semidim);
     }
     if constexpr (en.flags & VMAS_F_ROTATABLE) {
       if (sub == 0) r.w[e] = r.w[e] * en.drag_mult;

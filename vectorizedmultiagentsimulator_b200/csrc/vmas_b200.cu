@@ -160,8 +160,8 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
           }
           if (flg[j] & VMAS_F_F_RANGE) {
             const float r = __ldg(ef + VMAS_EF_F_RANGE);
-            afx[j] = fminf(fmaxf(afx[j], -r), r);
-            afy[j] = fminf(fmaxf(afy[j], -r), r);
+            afx[j] = clampf(afx[j], -r, r);
+            afy[j] = clampf(afy[j], -r, r);
           }
           Fx[j] = Fx[j] + afx[j];
           Fy[j] = Fy[j] + afy[j];
@@ -169,12 +169,12 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
         if (flg[j] & VMAS_F_ROTATABLE) {
           if (flg[j] & VMAS_F_MAX_T) {
             const float mx = __ldg(ef + VMAS_EF_MAX_T);
-            const float n = sqrtf(atq[j] * atq[j]);
+            const float n = fabsf(atq[j]);  // vector_norm of one element
             if (n > mx) atq[j] = (atq[j] / n) * mx;
           }
           if (flg[j] & VMAS_F_T_RANGE) {
             const float r = __ldg(ef + VMAS_EF_T_RANGE);
-            atq[j] = fminf(fmaxf(atq[j], -r), r);
+            atq[j] = clampf(atq[j], -r, r);
           }
           T[j] = T[j] + atq[j];
         }
@@ -188,7 +188,7 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
         }
       }
       if (flg[j] & VMAS_F_ANG_FRIC) {  // ref core.py:2089-2102
-        const float speed = sqrtf(w[j] * w[j]);
+        const float speed = fabsf(w[j]);  // vector_norm of one element
         if (speed != 0.f) {
           const float inertia = ent_inertia(a, flg[j], mass, ef);
           const float cap = ent_param(a, flg[j], VMAS_F_ANG_FRIC_ENV, env, e, VMAS_EP_ANG_FRIC, ef, VMAS_EF_ANG_FRIC) * inertia;
@@ -276,13 +276,13 @@ __global__ void __launch_bounds__(128) step_kernel(const StepArgs a) {
         }
         if (flg[j] & VMAS_F_V_RANGE) {
           const float r = __ldg(ef + VMAS_EF_V_RANGE);
-          vx[j] = fminf(fmaxf(vx[j], -r), r);
-          vy[j] = fminf(fmaxf(vy[j], -r), r);
+          vx[j] = clampf(vx[j], -r, r);
+          vy[j] = clampf(vy[j], -r, r);
         }
         px[j] = px[j] + vx[j] * sub_dt;
         py[j] = py[j] + vy[j] * sub_dt;
-        if (a.cfg.has_x_semidim) px[j] = fminf(fmaxf(px[j], -a.cfg.x_semidim), a.cfg.x_semidim);
-        if (a.cfg.has_y_semidim) py[j] = fminf(fmaxf(py[j], -a.cfg.y_semidim), a.cfg.y_semidim);
+        if (a.cfg.has_x_semidim) px[j] = clampf(px[j], -a.cfg.x_semidim, a.cfg.x_semidim);
+        if (a.cfg.has_y_semidim) py[j] = clampf(py[j], -a.cfg.y_semidim, a.cfg.y_semidim);
       }
       if (rotatable) {
         const float inertia =
