@@ -107,6 +107,8 @@ def test_device_tables_build_for_every_mapping_on_cpu():
             else:
                 with pytest.raises(RuntimeError):
                     _native.DeviceTables(tables, None, cpu, mapping=mapping)
+        with pytest.raises(ValueError, match="auto, specialized, tile, thread_per_env, lanes_per_env, block_per_env"):
+            _native.DeviceTables(tables, None, cpu, mapping="warp")
 
 
 def test_ctypes_structs_have_the_layout_of_the_c_header(tmp_path):

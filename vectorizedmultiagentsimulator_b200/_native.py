@@ -208,6 +208,8 @@ ENV_REORDER_MIN_BATCH = 1024  # below this there is nothing to gain from groupin
 ENV_REORDER_CHUNK = int(os.environ.get("VMAS_B200_ENV_REORDER_CHUNK", "2048"))  # envs sorted together
 #: what mapping="auto" picks for a specialised world that has both kernels
 DEFAULT_SPEC_MAPPING = os.environ.get("VMAS_B200_SPEC_MAPPING", "specialized")
+#: the values of ``DeviceTables(mapping=...)`` / ``VMAS_B200_MAPPING``
+MAPPINGS = ("auto", "specialized", "tile", "thread_per_env", "lanes_per_env", "block_per_env")
 
 
 class SpawnC(C.Structure):
@@ -460,7 +462,8 @@ class DeviceTables:
         self.device = torch.device(device)
         desc = tables.desc
         mapping = mapping or os.environ.get("VMAS_B200_MAPPING", "auto")
-        assert mapping in ("auto", "specialized", "tile", "thread_per_env", "lanes_per_env", "block_per_env"), mapping
+        if mapping not in MAPPINGS:
+            raise ValueError(f"unknown mapping {mapping!r}: expected one of {', '.join(MAPPINGS)}")
         if desc.n_entities > MAX_ENTITIES:
             raise NotImplementedError(
                 f"{desc.n_entities} entities per env exceed the CUDA backend's limit of {MAX_ENTITIES}"

@@ -97,8 +97,9 @@ def _seeded(method):
     return wrapper
 
 
-# opt-in (VMAS_B200_FORK_OBS=1): measured slower on balance / navigation / flocking at the BASELINE
-# batch sizes — the branches of the captured graph do not start together
+# opt-in (VMAS_B200_FORK_OBS=1): measured slower on balance / navigation / flocking at the BASELINE batch sizes
+# on a B200 — the branches of the captured graph do not start together; on an H100 it is faster on navigation
+# (DESIGN §7.3, §10)
 _FORK_OBSERVATIONS = os.environ.get("VMAS_B200_FORK_OBS", "0") == "1"
 
 
