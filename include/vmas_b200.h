@@ -329,6 +329,17 @@ int vmas_b200_set_l2_fetch_granularity(int32_t bytes);
  * tensors from every step, ref environment/environment.py:254-309).
  */
 int vmas_b200_copy_buffers(const VmasCopySegment* segs, int32_t n_segs, void* cuda_stream);
+/*
+ * The same, where segment i may convert: kinds[i] = VMAS_DTYPE_F32 copies `bytes` bytes as above;
+ * VMAS_DTYPE_F16 / VMAS_DTYPE_BF16 read `bytes` bytes of fp32 values (a multiple of 4, `src` 4-byte aligned) and
+ * write each rounded to nearest even to that 16-bit type (`bytes` / 2 bytes, `dst` 2-byte aligned): overflow goes
+ * to +-inf, -0 stays -0, a NaN stays NaN.  16-bit observations of a captured Environment.step are handed out so.
+ */
+#define VMAS_DTYPE_F32 0
+#define VMAS_DTYPE_F16 1
+#define VMAS_DTYPE_BF16 2
+int vmas_b200_copy_buffers_convert(const VmasCopySegment* segs, const int32_t* kinds, int32_t n_segs,
+                                   void* cuda_stream);
 
 
 /*
@@ -438,9 +449,9 @@ int vmas_b200_ingest_actions_broad_phase(const VmasWorldConfig* cfg, const VmasP
  *      callbacks, captured by the caller) is launched, or — `graph_exec` NULL — vmas_b200_world_step followed
  *      by vmas_b200_post_step (`program` / `columns` as there; both NULL: physics only) — or, with
  *      `fused_kernel`, ONE launch doing both;
- *   3. vmas_b200_copy_buffers handing results out: segment i is copied to out_blocks[seg_block[i]] +
- *      (byte offset held in segs[i].dst), so that a caller allocating fresh result blocks every step only
- *      fills in `out_blocks` (n_segs may be 0: see `obs_block` / `mirror_*` below).
+ *   3. vmas_b200_copy_buffers (with `seg_kind`: vmas_b200_copy_buffers_convert) handing results out: segment i is
+ *      copied to out_blocks[seg_block[i]] + (byte offset held in segs[i].dst), so that a caller allocating fresh
+ *      result blocks every step only fills in `out_blocks` (n_segs may be 0: see `obs_block` / `mirror_*` below).
  * `ingest_mask` non-NULL: the ingest launch also builds the first substep's broad-phase mask (then
  * `exact_broad_phase` must be 2 in direct mode, and the captured graph must have been captured that way).
  * Returns the number of kernels this call launched itself (the graph's nodes are not counted).
@@ -496,10 +507,16 @@ typedef struct VmasEnvStep {
    * ingest prologue for these agents (continuous holonomic actions) and the batch fits the GPU at once (a
    * masked world's broad phase needs a grid-wide barrier per substep; `mask` must then hold
    * substeps x ((n_masked + 31) / 32 + 2) zeroed words); otherwise the launches above are issued. */
-  int32_t ingest_in_kernel, reserved;
+  int32_t ingest_in_kernel;
+  /* what the post stage writes to out_blocks[obs_block] (obs_block >= 0; rows going to `obs_out` are fp32):
+   * VMAS_DTYPE_F32, or VMAS_DTYPE_F16 / VMAS_DTYPE_BF16 — each value rounded to nearest even; a `fused_kernel`
+   * must then have been compiled for that type */
+  int32_t obs_dtype;
   int32_t mirror_slot[VMAS_PROG_MAX_BUFFERS];
   int32_t mirror_block[VMAS_PROG_MAX_BUFFERS];
   size_t mirror_offset[VMAS_PROG_MAX_BUFFERS];
+  /* NULL, or n_segs kinds of the hand-out segments as vmas_b200_copy_buffers_convert takes them */
+  const int32_t* seg_kind;
 } VmasEnvStep;
 int vmas_b200_env_step(const VmasEnvStep* step, void* cuda_stream);
 

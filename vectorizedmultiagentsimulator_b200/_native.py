@@ -266,6 +266,7 @@ EXPORTS = [
     "vmas_b200_distance_shaping",
     "vmas_b200_post_step",
     "vmas_b200_copy_buffers",
+    "vmas_b200_copy_buffers_convert",
     "vmas_b200_env_step",
     "vmas_b200_register_step_kernel",
     "vmas_b200_graph_num_nodes",
@@ -337,6 +338,7 @@ def load():
     lib.vmas_b200_reset_state.argtypes = [p_cfg, p_st, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.vmas_b200_spawn_entities.argtypes = [p_cfg, p_st, C.POINTER(SpawnC), C.c_void_p]
     lib.vmas_b200_copy_buffers.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+    lib.vmas_b200_copy_buffers_convert.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     lib.vmas_b200_post_step.argtypes = [
         p_cfg, p_tb, p_st, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p
     ]
@@ -749,6 +751,10 @@ class CopySegmentC(C.Structure):
 
 
 MAX_COPY_SEGMENTS = 64
+#: element types of observation results (``VMAS_DTYPE_*``): what a converting copy segment writes, what the post
+#: stage stores; fp32 is a plain copy
+DTYPE_F32, DTYPE_F16, DTYPE_BF16 = 0, 1, 2
+DTYPE_CODES = {torch.float32: DTYPE_F32, torch.float16: DTYPE_F16, torch.bfloat16: DTYPE_BF16}
 
 
 def copy_buffers(lib, device, pairs) -> int:
@@ -764,13 +770,27 @@ def copy_buffers(lib, device, pairs) -> int:
     return n
 
 
+def _segment_kinds(items, block_kinds):
+    """``int32[n]`` kinds of the copy segments ``items`` = [(source, block, offset)] (``block_kinds[b]``: what
+    block ``b`` receives, ``DTYPE_F32`` = a plain copy), or None when every segment is a plain copy."""
+    if not block_kinds or not any(block_kinds[block] for _, block, _ in items):
+        return None
+    kinds = (C.c_int32 * len(items))()
+    for k, (src, block, _) in enumerate(items):
+        kinds[k] = block_kinds[block]
+        assert not kinds[k] or src.dtype == torch.float32, "a converting copy reads fp32"
+    return kinds
+
+
 class CopyPlan:
     """A fixed list of copies whose SOURCES never move (the buffers a captured step writes) into
     destination blocks that are allocated anew every step: sources, sizes and destination offsets are
     marshalled once, a run only adds the fresh base addresses."""
 
-    def __init__(self, items):
-        """``items``: [(source tensor (contiguous), destination block index, byte offset in that block)]."""
+    def __init__(self, items, block_kinds=None):
+        """``items``: [(source tensor (contiguous), destination block index, byte offset in that block)];
+        ``block_kinds``: per destination block, ``DTYPE_F16`` / ``DTYPE_BF16`` if its fp32 sources are to be
+        rounded to that type on the way (``DTYPE_F32`` or None: plain copies)."""
         assert len(items) <= MAX_COPY_SEGMENTS, f"at most {MAX_COPY_SEGMENTS} copies per plan"
         self.segs = (CopySegmentC * max(len(items), 1))()
         self.where = []
@@ -780,6 +800,7 @@ class CopyPlan:
             seg.src, seg.bytes = src.data_ptr(), src.numel() * src.element_size()
             self.where.append((block, offset))
         self.n = len(items)
+        self.kinds = _segment_kinds(items, block_kinds)
 
     def run(self, lib, device, bases) -> int:
         """``bases[i]``: address of destination block ``i``.  One launch."""
@@ -788,6 +809,8 @@ class CopyPlan:
         segs = self.segs
         for k, (block, offset) in enumerate(self.where):
             segs[k].dst = bases[block] + offset
+        if self.kinds is not None:
+            return _check(lib, lib.vmas_b200_copy_buffers_convert(segs, self.kinds, self.n, _stream(device)))
         return _check(lib, lib.vmas_b200_copy_buffers(segs, self.n, _stream(device)))
 
 
@@ -805,9 +828,10 @@ class EnvStepC(C.Structure):
         ("segs", C.c_void_p), ("seg_block", C.c_void_p), ("n_segs", C.c_int32), ("n_out_blocks", C.c_int32),
         ("out_blocks", C.c_void_p * MAX_OUT_BLOCKS),
         ("obs_block", C.c_int32), ("n_mirrors", C.c_int32), ("obs_offset", C.c_size_t),
-        ("ingest_in_kernel", C.c_int32), ("reserved", C.c_int32),
+        ("ingest_in_kernel", C.c_int32), ("obs_dtype", C.c_int32),
         ("mirror_slot", C.c_int32 * PROG_MAX_BUFFERS), ("mirror_block", C.c_int32 * PROG_MAX_BUFFERS),
         ("mirror_offset", C.c_size_t * PROG_MAX_BUFFERS),
+        ("seg_kind", C.c_void_p),
     ]
 
 
@@ -820,9 +844,10 @@ class EnvStepPlan:
     def __init__(self, lib, dt: "DeviceTables", slab, agents_c, n_agents: int, clamp: bool, bad_flag, steps,
                  ingest_broad_phase: bool, graph_exec: int, copy_items, n_out_blocks: int,
                  program=None, columns=None, n_rows: int = 0, width: int = 0, obs_out=None, exact_broad_phase: int = 1,
-                 obs_to=None, mirrors=()):
-        """``obs_to``: (block, byte offset) the observation rows are written to directly (direct mode);
-        ``mirrors``: [(program buffer slot, block, byte offset)] stores that land in the fresh blocks."""
+                 obs_to=None, mirrors=(), block_kinds=None, obs_dtype: int = DTYPE_F32):
+        """``obs_to``: (block, byte offset) the observation rows are written to directly (direct mode), as
+        ``obs_dtype`` (``DTYPE_*``); ``mirrors``: [(program buffer slot, block, byte offset)] stores that land in
+        the fresh blocks; ``block_kinds``: as ``CopyPlan`` takes them, for the hand-out copies."""
         assert len(copy_items) <= MAX_COPY_SEGMENTS and n_out_blocks <= MAX_OUT_BLOCKS and n_agents <= MAX_INGEST_AGENTS
         self.lib, self.device = lib, dt.device
         st = dt.state_struct(slab)
@@ -854,12 +879,15 @@ class EnvStepPlan:
         c.n_mirrors = len(mirrors)
         for k, (slot, block, offset) in enumerate(mirrors):
             c.mirror_slot[k], c.mirror_block[k], c.mirror_offset[k] = slot, block, offset
+        c.obs_dtype = obs_dtype if obs_to is not None else DTYPE_F32
+        kinds = _segment_kinds(copy_items, block_kinds)
+        c.seg_kind = None if kinds is None else C.addressof(kinds)
         self.out_blocks = c.out_blocks
         self.agents = agents_c
         self._ref = C.addressof(c)
         self._call = lib.vmas_b200_env_step
         # everything the addresses above point into stays alive with the plan
-        self.keep = (dt, slab, st, agents_c, segs, blocks, bad_flag, steps, program, columns, obs_out,
+        self.keep = (dt, slab, st, agents_c, segs, blocks, kinds, bad_flag, steps, program, columns, obs_out,
                      [src for src, _, _ in copy_items])
 
     def run(self) -> int:

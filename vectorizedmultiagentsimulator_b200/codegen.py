@@ -148,16 +148,18 @@ def emit_world(desc: P.WorldDescription, label: str, tuning: Dict = None) -> Tup
     return name, "\n".join(lines), h
 
 
-def post_hash(cols, instrs, acts=()) -> int:
+def post_hash(cols, instrs, acts=(), obs_dtype: int = 0) -> int:
     """FNV-1a 64 of what a whole-step kernel does around the substeps: the observation plan's column table
     (int32 ``[rows, width, 4]`` or None), the step program's instructions ``[(op, dst, a, b, arg, imm)]`` with
-    entity indices resolved, and the action ingest ``[(agent row, u_range x 2, u_multiplier x 2)]`` of the
-    policy agents (empty: actions are ingested by a launch of their own)."""
-    blob = json.dumps(
-        [None if cols is None else [list(cols.shape), [int(x) for x in cols.reshape(-1)]],
-         [[int(op), int(dst), int(a), int(b), int(arg), _f(imm)] for op, dst, a, b, arg, imm in instrs],
-         [[int(agent)] + [_f(v) for v in rest] for agent, *rest in acts]]
-    ).encode()
+    entity indices resolved, the action ingest ``[(agent row, u_range x 2, u_multiplier x 2)]`` of the
+    policy agents (empty: actions are ingested by a launch of their own) and the type of the observation rows
+    (``VMAS_DTYPE_*``; fp32 adds nothing to the hash)."""
+    parts = [None if cols is None else [list(cols.shape), [int(x) for x in cols.reshape(-1)]],
+             [[int(op), int(dst), int(a), int(b), int(arg), _f(imm)] for op, dst, a, b, arg, imm in instrs],
+             [[int(agent)] + [_f(v) for v in rest] for agent, *rest in acts]]
+    if obs_dtype:
+        parts.append(int(obs_dtype))
+    blob = json.dumps(parts).encode()
     h = 0xCBF29CE484222325
     for byte in blob:
         h ^= byte
@@ -180,14 +182,18 @@ def fuse_value_columns(cols, buffer_sources, instrs):
     return cols
 
 
-def emit_post(cols, instrs, acts=()) -> Tuple[str, str, int]:
+def emit_post(cols, instrs, acts=(), obs_dtype: int = 0) -> Tuple[str, str, int]:
     """C++ text of one epilogue (+ ingest prologue) struct (``spec_epilogue`` / ``spec_ingest`` in
-    csrc/spec_kernel.cuh).  Returns (name, text, hash)."""
-    h = post_hash(cols, instrs, acts)
+    csrc/spec_kernel.cuh).  ``obs_dtype``: what the observation rows are stored as (``VMAS_DTYPE_F32`` = 0,
+    ``VMAS_DTYPE_F16`` = 1, ``VMAS_DTYPE_BF16`` = 2).  Returns (name, text, hash)."""
+    h = post_hash(cols, instrs, acts, obs_dtype)
     name = f"Post_{h:016x}"
     rows, width = (0, 0) if cols is None else (int(cols.shape[0]), int(cols.shape[1]))
     lines = [f"struct {name} {{"]
-    lines.append(f"  static constexpr int N_PROG = {len(instrs)}, OBS_ROWS = {rows}, OBS_WIDTH = {width}, N_ACT = {len(acts)};")
+    lines.append(
+        f"  static constexpr int N_PROG = {len(instrs)}, OBS_ROWS = {rows}, OBS_WIDTH = {width}, N_ACT = {len(acts)}, "
+        f"OBS_DTYPE = {int(obs_dtype)};"
+    )
     lines.append(f"  static constexpr ActC act[{max(len(acts), 1)}] = {{")
     for agent, r0, r1, m0, m1 in acts:
         lines.append(f"      {{{int(agent)}, {_f(r0)}, {_f(r1)}, {_f(m0)}, {_f(m1)}}},")

@@ -9,10 +9,79 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stdint.h>
+#ifdef __CUDACC__
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#endif
 
 #define DEVI __device__ __forceinline__
 
 namespace vmas {
+
+// 16-bit observation values (VMAS_DTYPE_F16 / VMAS_DTYPE_BF16): fp32 -> the bits of the 16-bit value, rounded to
+// nearest even by the hardware conversion (cvt.rn.f16.f32 / cvt.rn.bf16.f32, packed pairs as cvt.rn.*x2.f32):
+// overflow goes to +-inf, -0 stays -0, NaN stays NaN.  x2: `lo` in the low half (the lower address).  The host
+// build (tests/hostsim) spells out the same rounding; NaN payloads may differ from the device's.
+DEVI uint16_t f16_bits(float v) {
+#ifdef __CUDA_ARCH__
+  return __half_as_ushort(__float2half_rn(v));
+#else
+  const uint32_t x = __float_as_uint(v), ax = x & 0x7FFFFFFFu;
+  const uint16_t sign = (uint16_t)((x >> 16) & 0x8000u);
+  if (ax > 0x7F800000u) return (uint16_t)(sign | 0x7E00u | ((ax >> 13) & 0x3FFu));
+  if (ax >= 0x477FF000u) return (uint16_t)(sign | 0x7C00u);  // >= 65520: the tie above 65504 rounds to inf
+  if (ax >= 0x38800000u) {                                  // normal: re-bias the exponent, round 13 bits
+    const uint32_t r = ax - 0x38000000u;
+    return (uint16_t)(sign | ((r + 0xFFFu + ((r >> 13) & 1u)) >> 13));
+  }
+  const int e = (int)(ax >> 23);  // subnormal (or zero) in units of 2^-24
+  const int shift = 126 - e;
+  if (e == 0 || shift > 24) return sign;
+  const uint32_t m = (ax & 0x7FFFFFu) | 0x800000u;
+  uint32_t q = m >> shift;
+  const uint32_t rem = m & ((1u << shift) - 1u), half = 1u << (shift - 1);
+  if (rem > half || (rem == half && (q & 1u))) ++q;
+  return (uint16_t)(sign | q);
+#endif
+}
+DEVI uint16_t bf16_bits(float v) {
+#ifdef __CUDA_ARCH__
+  return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+#else
+  const uint32_t x = __float_as_uint(v);
+  if ((x & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((x >> 16) | 0x40u);
+  return (uint16_t)((x + 0x7FFFu + ((x >> 16) & 1u)) >> 16);
+#endif
+}
+DEVI uint32_t f16x2_bits(float lo, float hi) {
+#ifdef __CUDA_ARCH__
+  const __half2 h = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&h);
+#else
+  return (uint32_t)f16_bits(lo) | ((uint32_t)f16_bits(hi) << 16);
+#endif
+}
+DEVI uint32_t bf16x2_bits(float lo, float hi) {
+#ifdef __CUDA_ARCH__
+  const __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&h);
+#else
+  return (uint32_t)bf16_bits(lo) | ((uint32_t)bf16_bits(hi) << 16);
+#endif
+}
+template <int DT>
+DEVI uint16_t obs16_bits(float v) {
+  static_assert(DT == 1 || DT == 2, "16-bit observation dtypes: VMAS_DTYPE_F16, VMAS_DTYPE_BF16");
+  if constexpr (DT == 1) return f16_bits(v);
+  else return bf16_bits(v);
+}
+template <int DT>
+DEVI uint32_t obs16x2_bits(float lo, float hi) {
+  static_assert(DT == 1 || DT == 2, "16-bit observation dtypes: VMAS_DTYPE_F16, VMAS_DTYPE_BF16");
+  if constexpr (DT == 1) return f16x2_bits(lo, hi);
+  else return bf16x2_bits(lo, hi);
+}
 
 struct V2 {
   float x, y;

@@ -50,7 +50,7 @@ struct ObsColC {
   float par;
 };
 struct EpiArgs {
-  float* obs_out;  // [rows, B, width] or null
+  void* obs_out;  // [rows, B, width] of P::OBS_DTYPE (fp32, fp16 or bf16), or null
   void* buffers[VMAS_PROG_MAX_BUFFERS];
 };
 // ... and its prologue (see spec_ingest): the policy agents' continuous holonomic actions
@@ -972,17 +972,22 @@ DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs
         static_cast<uint8_t*>(e.buffers[in.b])[env] = pr[in.a] != 0.f ? 1 : 0;
     }
   });
-  // the observation rows (ref scenarios/balance.py:236-262 as an ObservationPlan): [rows, B, width]
+  // the observation rows (ref scenarios/balance.py:236-262 as an ObservationPlan): [rows, B, width] of
+  // P::OBS_DTYPE.  16-bit rows are rounded here, in registers, pair by pair as the values come, and stored as one
+  // 4-byte word per pair: 8-byte stores of 4 columns cost the lane-pair kernel of balance a register (127, not 126)
   if constexpr (P::OBS_ROWS > 0) {
-    constexpr int F = P::OBS_WIDTH;
-    constexpr int VEC = F % 4 == 0 ? 4 : 1;
+    constexpr int DT = P::OBS_DTYPE, F = P::OBS_WIDTH;
+    constexpr int VEC = DT != VMAS_DTYPE_F32 ? (F % 2 == 0 ? 2 : 1) : F % 4 == 0 ? 4 : 1;
     static_for<P::OBS_ROWS>([&](auto ri) {
       constexpr int row = decltype(ri)::value;
       if (lane != row % lanes) return;
-      float* dst = e.obs_out + ((size_t)row * a.batch_dim + env) * F;
+      const size_t at = ((size_t)row * a.batch_dim + env) * F;
+      float* dst = static_cast<float*>(e.obs_out) + at;
+      uint16_t* dst16 = static_cast<uint16_t*>(e.obs_out) + at;
       static_for<F / VEC>([&](auto gi) {
         constexpr int c0 = decltype(gi)::value * VEC;
         float v[VEC];
+        [[maybe_unused]] uint32_t packed[VEC / 2 > 0 ? VEC / 2 : 1];
         bool all = true;
         static_for<VEC>([&](auto ki) {
           constexpr int k = decltype(ki)::value;
@@ -998,16 +1003,27 @@ DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs
           } else {
             all = false;
           }
+          if constexpr (DT != VMAS_DTYPE_F32 && k % 2 == 1) packed[k / 2] = obs16x2_bits<DT>(v[k - 1], v[k]);
         });
-        if constexpr (VEC == 4) {
+        if constexpr (DT == VMAS_DTYPE_F32) {
+          if constexpr (VEC == 4) {
+            if (all) {
+              *reinterpret_cast<float4*>(dst + c0) = make_float4(v[0], v[1], v[2], v[3]);
+              return;
+            }
+          }
+        } else if constexpr (VEC == 2) {
           if (all) {
-            *reinterpret_cast<float4*>(dst + c0) = make_float4(v[0], v[1], v[2], v[3]);
+            *reinterpret_cast<uint32_t*>(dst16 + c0) = packed[0];
             return;
           }
         }
         static_for<VEC>([&](auto ki) {
           constexpr int k = decltype(ki)::value;
-          if constexpr (P::obs[row * F + c0 + k].op != VMAS_OBS_SKIP) dst[c0 + k] = v[k];
+          if constexpr (P::obs[row * F + c0 + k].op != VMAS_OBS_SKIP) {
+            if constexpr (DT == VMAS_DTYPE_F32) dst[c0 + k] = v[k];
+            else dst16[c0 + k] = obs16_bits<DT>(v[k]);
+          }
         });
       });
     });

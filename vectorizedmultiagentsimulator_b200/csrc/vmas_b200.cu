@@ -877,7 +877,7 @@ __global__ void __launch_bounds__(256) point_query_kernel(const QueryArgs q) {
 struct ObsArgs {
   VmasState st;
   const int32_t* cols;  // [rows * width * 4]
-  float* out;           // [rows, B, width]
+  void* out;            // [rows, B, width] of the launch's DT (fp32, or fp16 / bf16 rounded to nearest even)
   int32_t rows, width, batch_dim, n_entities;
   const float* buffers[VMAS_OBS_MAX_BUFFERS];  // VMAS_OBS_BUFFER columns: fp32 [B] each
 };
@@ -896,8 +896,9 @@ struct ObsSrc {
 // (2) threadIdx.x = a group of VEC adjacent columns, threadIdx.y = env lane: a thread decodes its
 //     columns once (shared-memory offsets in registers) and walks the tile's envs; per env a
 //     handful of shared-memory loads, at most one subtraction per column and one vector store;
-//     consecutive lanes write consecutive pieces of an env's output row.
-template <int VEC>
+//     consecutive lanes write consecutive pieces of an env's output row.  DT != VMAS_DTYPE_F32: the values are
+//     rounded to 16 bits in registers and stored at half the width (4 columns: one 8-byte store).
+template <int VEC, int DT = VMAS_DTYPE_F32>
 DEVI void gather_observations_body(const ObsArgs& a, const int tile_envs, const int obs_row) {
   extern __shared__ float4 s_state4[];
   float* s_state = reinterpret_cast<float*>(s_state4);
@@ -956,7 +957,7 @@ DEVI void gather_observations_body(const ObsArgs& a, const int tile_envs, const 
     all &= c.x != VMAS_OBS_SKIP;
   }
   if (g >= groups || !any) return;  // columns owned by another producer (LIDAR, the scenario)
-  float* out = a.out + ((size_t)row * a.batch_dim + env0) * a.width + g * VEC;
+  const size_t out_at = ((size_t)row * a.batch_dim + env0) * a.width + g * VEC;
   for (unsigned e = threadIdx.y; e < n_env; e += blockDim.y) {
     float v[VEC];
 #pragma unroll
@@ -970,19 +971,34 @@ DEVI void gather_observations_body(const ObsArgs& a, const int tile_envs, const 
         if (op[k] == VMAS_OBS_REMAINDER) v[k] = obs_remainder(v[k], par[k]);
       }
     }
-    float* dst = out + (size_t)e * a.width;
-    if (all) {
-      if constexpr (VEC == 4) {
-        *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-      } else if constexpr (VEC == 2) {
-        *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
+    if constexpr (DT == VMAS_DTYPE_F32) {
+      float* dst = static_cast<float*>(a.out) + out_at + (size_t)e * a.width;
+      if (all) {
+        if constexpr (VEC == 4) {
+          *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+        } else if constexpr (VEC == 2) {
+          *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
+        } else {
+          dst[0] = v[0];
+        }
       } else {
-        dst[0] = v[0];
+#pragma unroll
+        for (int k = 0; k < VEC; ++k)
+          if (op[k] != VMAS_OBS_SKIP) dst[k] = v[k];
       }
     } else {
+      uint16_t* dst = static_cast<uint16_t*>(a.out) + out_at + (size_t)e * a.width;
+      if (all && VEC > 1) {
+        if constexpr (VEC == 4) {
+          *reinterpret_cast<uint2*>(dst) = make_uint2(obs16x2_bits<DT>(v[0], v[1]), obs16x2_bits<DT>(v[2], v[3]));
+        } else if constexpr (VEC == 2) {
+          *reinterpret_cast<uint32_t*>(dst) = obs16x2_bits<DT>(v[0], v[1]);
+        }
+      } else {
 #pragma unroll
-      for (int k = 0; k < VEC; ++k)
-        if (op[k] != VMAS_OBS_SKIP) dst[k] = v[k];
+        for (int k = 0; k < VEC; ++k)
+          if (op[k] != VMAS_OBS_SKIP) dst[k] = obs16_bits<DT>(v[k]);
+      }
     }
   }
 }
@@ -1083,13 +1099,13 @@ DEVI void post_step_program_body(const ProgArgs& p, const int tile_envs) {
 
 // blockIdx.y == 0 (when there is a program): the program blocks — scheduled first, because a program thread
 // is a chain of dependent queries (latency) that the bandwidth-bound gather blocks behind it can hide
-template <int VEC>
+template <int VEC, int DT = VMAS_DTYPE_F32>
 __global__ void __launch_bounds__(256, 5) post_step_kernel(const ObsArgs obs, const int tile_envs, const ProgArgs prog) {
   const int first_obs = prog.prog.n_instr > 0 ? 1 : 0;
   if ((int)blockIdx.y < first_obs)
     post_step_program_body(prog, tile_envs);
   else
-    gather_observations_body<VEC>(obs, tile_envs, (int)blockIdx.y - first_obs);
+    gather_observations_body<VEC, DT>(obs, tile_envs, (int)blockIdx.y - first_obs);
 }
 
 template <bool KIN>
@@ -1360,6 +1376,63 @@ __global__ void __launch_bounds__(256) copy_buffers_kernel(const CopyArgs a, con
   const VmasCopySegment s = a.seg[k];
   const size_t n_blocks = (size_t)(a.first_block[k + 1] - a.first_block[k]);
   const size_t tid = (size_t)(blockIdx.x - a.first_block[k]) * blockDim.x + threadIdx.x, stride = n_blocks * blockDim.x;
+  const char* src = static_cast<const char*>(s.src);
+  char* dst = static_cast<char*>(s.dst);
+  size_t done = 0;
+  if ((((uintptr_t)src | (uintptr_t)dst) & 15u) == 0) {
+    const size_t words = s.bytes / 16;
+    const uint4* s4 = reinterpret_cast<const uint4*>(src);
+    uint4* d4 = reinterpret_cast<uint4*>(dst);
+    for (size_t i = tid; i < words; i += stride) d4[i] = s4[i];
+    done = words * 16;
+  }
+  for (size_t i = done + tid; i < s.bytes; i += stride) dst[i] = src[i];
+}
+
+struct CopyKinds {
+  int32_t kind[VMAS_MAX_COPY_SEGMENTS];  // VMAS_DTYPE_F32: a byte copy; VMAS_DTYPE_F16 / _BF16: fp32 -> 16 bit
+};
+
+// fp32 [n] -> 16-bit [n], rounded to nearest even: the elements in front of the first 16-byte aligned source
+// word one by one, then 16-byte loads and 8-byte stores (when the destination is 8-byte aligned there too; the
+// two pointers advance 4 : 2 bytes per element, so that holds for all words or none), the tail one by one
+template <int DT>
+DEVI void convert_segment(const float* src, uint16_t* dst, const size_t n, const size_t tid, const size_t stride) {
+  size_t head = (size_t)((16u - ((uintptr_t)src & 15u)) & 15u) / 4u;
+  if (head > n) head = n;
+  size_t done = n;
+  if ((((uintptr_t)(dst + head)) & 7u) == 0) {
+    const size_t words = (n - head) / 4;
+    const float4* s4 = reinterpret_cast<const float4*>(src + head);
+    uint2* d2 = reinterpret_cast<uint2*>(dst + head);
+    for (size_t i = tid; i < words; i += stride) {
+      const float4 v = s4[i];
+      d2[i] = make_uint2(obs16x2_bits<DT>(v.x, v.y), obs16x2_bits<DT>(v.z, v.w));
+    }
+    for (size_t i = tid; i < head; i += stride) dst[i] = obs16_bits<DT>(src[i]);
+    done = head + words * 4;
+  } else {
+    done = 0;
+  }
+  for (size_t i = done + tid; i < n; i += stride) dst[i] = obs16_bits<DT>(src[i]);
+}
+
+// copy_buffers_kernel with converting segments: the same split of the blocks over the segments
+__global__ void __launch_bounds__(256) copy_convert_kernel(const CopyArgs a, const CopyKinds kinds, const int n_segs) {
+  int k = 0;
+  while (k + 1 < n_segs && (int)blockIdx.x >= a.first_block[k + 1]) ++k;
+  const VmasCopySegment s = a.seg[k];
+  const size_t n_blocks = (size_t)(a.first_block[k + 1] - a.first_block[k]);
+  const size_t tid = (size_t)(blockIdx.x - a.first_block[k]) * blockDim.x + threadIdx.x, stride = n_blocks * blockDim.x;
+  const int kind = kinds.kind[k];
+  if (kind == VMAS_DTYPE_F16) {
+    convert_segment<VMAS_DTYPE_F16>(static_cast<const float*>(s.src), static_cast<uint16_t*>(s.dst), s.bytes / 4, tid, stride);
+    return;
+  }
+  if (kind == VMAS_DTYPE_BF16) {
+    convert_segment<VMAS_DTYPE_BF16>(static_cast<const float*>(s.src), static_cast<uint16_t*>(s.dst), s.bytes / 4, tid, stride);
+    return;
+  }
   const char* src = static_cast<const char*>(s.src);
   char* dst = static_cast<char*>(s.dst);
   size_t done = 0;
@@ -1799,10 +1872,21 @@ int vmas_b200_gather_observations_buffers(const VmasWorldConfig* cfg, const Vmas
   return 1;
 }
 
-int vmas_b200_post_step(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,
-                        const VmasStepProgram* program, const int32_t* columns, int32_t n_rows, int32_t width,
-                        float* obs_out, void* cuda_stream) {
+}  // extern "C"
+
+template <int VEC>
+static auto post_step_kernel_of(int obs_dtype) {
+  return obs_dtype == VMAS_DTYPE_F16 ? post_step_kernel<VEC, VMAS_DTYPE_F16>
+         : obs_dtype == VMAS_DTYPE_BF16 ? post_step_kernel<VEC, VMAS_DTYPE_BF16>
+                                        : post_step_kernel<VEC, VMAS_DTYPE_F32>;
+}
+
+// vmas_b200_post_step with the observation rows stored as `obs_dtype` (VMAS_DTYPE_*)
+static int post_step_impl(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,
+                          const VmasStepProgram* program, const int32_t* columns, int32_t n_rows, int32_t width,
+                          void* obs_out, int obs_dtype, void* cuda_stream) {
   if (check_common(cfg, tb, st) < 0) return -1;
+  if (obs_dtype < VMAS_DTYPE_F32 || obs_dtype > VMAS_DTYPE_BF16) return fail("unknown observation dtype%s");
   const bool has_prog = program && program->n_instr > 0, has_obs = columns && n_rows > 0;
   if (!has_prog && !has_obs) return fail("neither a program nor observation rows%s");
   if (has_prog && (program->n_instr > VMAS_PROG_MAX_INSTR)) return fail("program too long%s");
@@ -1835,7 +1919,11 @@ int vmas_b200_post_step(const VmasWorldConfig* cfg, const VmasPlanTables* tb, co
   for (int i = 0; i < VMAS_OBS_MAX_BUFFERS; ++i) oa.buffers[i] = nullptr;  // (buffer columns need a launch of their own)
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   int vec = 4;
-  if (has_obs) vec = (width % 4 == 0 && ((uintptr_t)obs_out % 16 == 0)) ? 4 : (width % 2 == 0 && ((uintptr_t)obs_out % 8 == 0)) ? 2 : 1;
+  if (has_obs) {
+    // 16-bit rows: the same groups of columns, stores of half the size
+    const uintptr_t a16 = obs_dtype == VMAS_DTYPE_F32 ? 16 : 8, a8 = obs_dtype == VMAS_DTYPE_F32 ? 8 : 4;
+    vec = (width % 4 == 0 && ((uintptr_t)obs_out % a16 == 0)) ? 4 : (width % 2 == 0 && ((uintptr_t)obs_out % a8 == 0)) ? 2 : 1;
+  }
   const int groups = oa.width / vec;
   if (groups > 256 || groups < 1) return fail("observation rows wider than 1024 columns are not supported%s");
   const unsigned bx = (unsigned)groups, by = 256 / bx;
@@ -1844,11 +1932,19 @@ int vmas_b200_post_step(const VmasWorldConfig* cfg, const VmasPlanTables* tb, co
   size_t smem = 0;
   if (obs_tile(cfg->n_entities, &tile, &smem) < 0) return -1;
   const dim3 grid((unsigned)((cfg->batch_dim + tile - 1) / tile), (unsigned)(oa.rows + (has_prog ? 1 : 0)));
-  auto kern = vec == 4 ? post_step_kernel<4> : vec == 2 ? post_step_kernel<2> : post_step_kernel<1>;
+  auto kern = vec == 4 ? post_step_kernel_of<4>(obs_dtype) : vec == 2 ? post_step_kernel_of<2>(obs_dtype) : post_step_kernel_of<1>(obs_dtype);
   if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, block, smem, stream>>>(oa, tile, pa);
   CUDA_OK(cudaGetLastError());
   return 1;
+}
+
+extern "C" {
+
+int vmas_b200_post_step(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,
+                        const VmasStepProgram* program, const int32_t* columns, int32_t n_rows, int32_t width,
+                        float* obs_out, void* cuda_stream) {
+  return post_step_impl(cfg, tb, st, program, columns, n_rows, width, obs_out, VMAS_DTYPE_F32, cuda_stream);
 }
 
 int vmas_b200_pair_query_batched(const VmasWorldConfig* cfg, const VmasPlanTables* tb, const VmasState* st,
@@ -1958,6 +2054,33 @@ int vmas_b200_copy_buffers(const VmasCopySegment* segs, int32_t n_segs, void* cu
   return 1;
 }
 
+int vmas_b200_copy_buffers_convert(const VmasCopySegment* segs, const int32_t* kinds, int32_t n_segs,
+                                   void* cuda_stream) {
+  if (!segs || !kinds || n_segs <= 0 || n_segs > VMAS_MAX_COPY_SEGMENTS) return fail("1..VMAS_MAX_COPY_SEGMENTS segments expected%s");
+  CopyArgs a;
+  CopyKinds k;
+  const int threads = 256;
+  const size_t per_block = (size_t)threads * 4 * 16;  // ~4 x 16 B (of the source) per thread
+  int blocks = 0;
+  for (int i = 0; i < n_segs; ++i) {
+    if (!segs[i].src || !segs[i].dst) return fail("null copy segment%s");
+    if (kinds[i] < VMAS_DTYPE_F32 || kinds[i] > VMAS_DTYPE_BF16) return fail("unknown copy segment kind%s");
+    if (kinds[i] != VMAS_DTYPE_F32 &&
+        (segs[i].bytes % 4 || ((uintptr_t)segs[i].src & 3u) || ((uintptr_t)segs[i].dst & 1u)))
+      return fail("a converting segment needs whole fp32 values at 4-byte aligned sources, 2-byte aligned destinations%s");
+    a.seg[i] = segs[i];
+    k.kind[i] = kinds[i];
+    a.first_block[i] = blocks;
+    size_t want = (segs[i].bytes + per_block - 1) / per_block;
+    want = want < 1 ? 1 : (want > 132 * 8 ? 132 * 8 : want);  // at most 8 blocks per SM of an H100 SXM
+    blocks += (int)want;
+  }
+  a.first_block[n_segs] = blocks;
+  copy_convert_kernel<<<(unsigned)blocks, threads, 0, static_cast<cudaStream_t>(cuda_stream)>>>(a, k, n_segs);
+  CUDA_OK(cudaGetLastError());
+  return 1;
+}
+
 int vmas_b200_graph_num_nodes(void* cuda_graph) {
   if (!cuda_graph) return fail("null graph%s");
   size_t n = 0;
@@ -1971,17 +2094,21 @@ int vmas_b200_graph_num_nodes(void* cuda_graph) {
 
 // where this step's post stage writes: the caller's static buffers, or (direct mode) this step's fresh blocks
 struct StepTargets {
-  float* obs_out;
+  void* obs_out;
+  int obs_dtype;  // of obs_out: s->obs_dtype in the caller's fresh block, fp32 in the static buffer
   const VmasStepProgram* program;
   VmasStepProgram patched;
 };
 
 static int env_step_targets(const VmasEnvStep* s, StepTargets& t) {
   t.obs_out = s->obs_out;
+  t.obs_dtype = VMAS_DTYPE_F32;
   t.program = s->program;
+  if (s->obs_dtype < VMAS_DTYPE_F32 || s->obs_dtype > VMAS_DTYPE_BF16) return fail("unknown observation dtype%s");
   if (s->obs_block >= 0 && s->columns && s->n_rows > 0) {
     if (s->obs_block >= s->n_out_blocks || !s->out_blocks[s->obs_block]) return fail("observation rows without their block%s");
-    t.obs_out = reinterpret_cast<float*>(static_cast<char*>(s->out_blocks[s->obs_block]) + s->obs_offset);
+    t.obs_out = static_cast<char*>(s->out_blocks[s->obs_block]) + s->obs_offset;
+    t.obs_dtype = s->obs_dtype;
   }
   if (s->n_mirrors > 0) {
     if (!s->program || s->n_mirrors > VMAS_PROG_MAX_BUFFERS) return fail("mirrored stores without a program%s");
@@ -2010,6 +2137,7 @@ static int env_step_hand_out(const VmasEnvStep* s, void* cuda_stream) {
     segs[i].dst = static_cast<char*>(s->out_blocks[b]) + reinterpret_cast<uintptr_t>(s->segs[i].dst);
     segs[i].bytes = s->segs[i].bytes;
   }
+  if (s->seg_kind) return vmas_b200_copy_buffers_convert(segs, s->seg_kind, s->n_segs, cuda_stream);
   return vmas_b200_copy_buffers(segs, s->n_segs, cuda_stream);
 }
 
@@ -2101,8 +2229,8 @@ int vmas_b200_env_step(const VmasEnvStep* s, void* cuda_stream) {
         if (r < 0) return r;
         launches += r;
         if (has_post) {
-          r = vmas_b200_post_step(s->cfg, s->tb, s->st, t.program, s->columns, s->n_rows, s->width, t.obs_out,
-                                  cuda_stream);
+          r = post_step_impl(s->cfg, s->tb, s->st, t.program, s->columns, s->n_rows, s->width, t.obs_out, t.obs_dtype,
+                             cuda_stream);
           if (r < 0) return r;
           launches += r;
         }

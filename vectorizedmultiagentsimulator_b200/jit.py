@@ -196,16 +196,16 @@ class StepKernelJob(Job):
     """The whole-step kernel of one (world, observation columns, step program): ``index`` is the handle for
     ``VmasEnvStep.fused_kernel`` once ``done`` is set."""
 
-    def __init__(self, desc: P.WorldDescription, cols, instrs, acts=(), out_dir: Optional[str] = None):
+    def __init__(self, desc: P.WorldDescription, cols, instrs, acts=(), out_dir: Optional[str] = None, obs_dtype: int = 0):
         super().__init__(desc, out_dir)
-        self.cols, self.instrs, self.acts = cols, instrs, tuple(acts)
-        self.post_hash = codegen.post_hash(cols, instrs, self.acts)
+        self.cols, self.instrs, self.acts, self.obs_dtype = cols, instrs, tuple(acts), int(obs_dtype)
+        self.post_hash = codegen.post_hash(cols, instrs, self.acts, self.obs_dtype)
         self.key = (self.hash ^ ((self.post_hash << 1) | (self.post_hash >> 63))) & 0xFFFFFFFFFFFFFFFF
 
     def _compile_and_register(self) -> int:
         desc = self.desc
         name, text, h = codegen.emit_world(desc, "whole-step kernel")
-        post_name, post_text, _ = codegen.emit_post(self.cols, self.instrs, self.acts)
+        post_name, post_text, _ = codegen.emit_post(self.cols, self.instrs, self.acts, self.obs_dtype)
         stem = f"step_{self.key:016x}_{_native.ARITH}_{_source_stamp()}"
         source = _STEP_TEMPLATE.format(world=text, post=post_text, name=name, post_name=post_name)
         obj = C.CDLL(_shared_object(stem, source, self.out_dir))
@@ -225,14 +225,16 @@ class StepKernelJob(Job):
 _step_jobs: Dict[int, StepKernelJob] = {}
 
 
-def request_step_kernel(desc: P.WorldDescription, cols, instrs, acts=(), block: bool = False) -> Optional[StepKernelJob]:
+def request_step_kernel(desc: P.WorldDescription, cols, instrs, acts=(), block: bool = False,
+                        obs_dtype: int = 0) -> Optional[StepKernelJob]:
     """Starts (or finds) the compilation of the whole-step kernel; None if the world cannot be specialised or
     has per-env physical parameters (those step on the captured graph of the specialised substep kernel).
     ``acts``: [(agent row, u_range x 2, u_multiplier x 2)] of the policy agents if the kernel is to ingest
-    their (continuous, holonomic) actions itself."""
+    their (continuous, holonomic) actions itself.  ``obs_dtype``: the type the kernel stores its observation
+    rows as (``VMAS_DTYPE_*``; part of the key)."""
     if not available() or not codegen.specializable(desc):
         return None
-    job = StepKernelJob(desc, cols, instrs, acts)
+    job = StepKernelJob(desc, cols, instrs, acts, obs_dtype=obs_dtype)
     with _lock:
         have = _step_jobs.get(job.key)
         if have is None:

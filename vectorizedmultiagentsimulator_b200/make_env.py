@@ -3,8 +3,11 @@ from __future__ import annotations
 
 from typing import Optional, Union
 
+import torch
+
 from . import scenarios
 from .simulator.environment import Environment, Wrapper
+from .simulator.environment.environment import check_obs_dtype
 from .simulator.scenario import BaseScenario
 from .simulator.utils import DEVICE_TYPING
 
@@ -26,6 +29,7 @@ def make_env(
     cuda_graph: bool = False,
     action_checks: Optional[str] = None,
     auto_reset: bool = False,
+    obs_dtype: torch.dtype = torch.float32,
     **kwargs,
 ):
     """Create a vectorised environment.
@@ -37,8 +41,13 @@ def make_env(
     ``cuda_graph=True`` replays one captured CUDA graph per ``step`` (graph-safe scenarios only),
     ``action_checks`` selects ``"sync"`` / ``"deferred"`` / ``"off"`` validation of the input
     actions, ``auto_reset=True`` resets finished envs on the device inside ``step`` (see
-    ``Environment``).  Remaining ``kwargs`` go to ``Scenario.make_world``.
+    ``Environment``), ``obs_dtype`` (``torch.float32``, ``torch.float16`` or ``torch.bfloat16``) is the type
+    every fp32 observation leaf is handed out as.  Remaining ``kwargs`` go to ``Scenario.make_world``.
     """
+    check_obs_dtype(obs_dtype)
+    if wrapper is not None and obs_dtype == torch.bfloat16:
+        raise ValueError("obs_dtype=torch.bfloat16 cannot be combined with a wrapper: the adapters convert "
+                         "observations to numpy, which has no bfloat16 (torch.float16 works)")
     env = Environment(
         _as_scenario(scenario),
         num_envs=num_envs,
@@ -56,6 +65,7 @@ def make_env(
         cuda_graph=cuda_graph,
         action_checks=action_checks,
         auto_reset=auto_reset,
+        obs_dtype=obs_dtype,
         **kwargs,
     )
     if wrapper is None:

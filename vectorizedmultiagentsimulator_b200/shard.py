@@ -55,19 +55,20 @@ def aggregate_throughput(local_units: float, local_seconds: float, device=None) 
     return sum_over_ranks(local_units, device) / max_over_ranks(local_seconds, device)
 
 
-def make_shard_env(scenario, total_envs: int, rank: int, world_size: int, device, seed: int = 0, **kwargs):
+def make_shard_env(scenario, total_envs: int, rank: int, world_size: int, device, seed: int = 0,
+                   obs_dtype: torch.dtype = torch.float32, **kwargs):
     """This rank's shard of a job of ``total_envs`` envs: ``make_env`` with the shard's size, plus
     the shard's position in the job (``world.env_offset``) so that every reset — including the one
     that builds the initial state — places entities exactly where the unsharded job would place
     them for the same envs (the respawn kernel numbers its random streams by global env index).
     That holds for scenarios whose reset draws all come from ``ScenarioUtils`` / ``World.spawn_positions``
     (the four shipped ones); draws taken from torch's generator are reproducible per shard but differ
-    from the unsharded job's.
+    from the unsharded job's.  ``obs_dtype``: as ``make_env`` takes it.
     """
     from .make_env import make_env
 
     lo, hi = shard_bounds(total_envs, rank, world_size)
-    env = make_env(scenario, num_envs=hi - lo, device=device, seed=seed, **kwargs)
+    env = make_env(scenario, num_envs=hi - lo, device=device, seed=seed, obs_dtype=obs_dtype, **kwargs)
     env.world.env_offset = lo
     env.world.reset_count.zero_()  # the construction-time reset above does not count as an episode
     env.reset(seed=seed)

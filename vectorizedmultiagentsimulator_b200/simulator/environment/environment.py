@@ -13,6 +13,9 @@ with one ``[num_envs, ...]`` tensor per policy agent).  What differs is undernea
   ``rewards / dones / infos`` describe the step that ended the episode, ``obs`` of a finished env is
   the first observation of its next episode — what ``obs = env.reset_at(dones)`` after the step
   would return, without the host in the loop (and, in graph mode, inside the captured graph);
+* ``obs_dtype=torch.float16 | torch.bfloat16`` (extension) hands observations out as 16-bit values: every fp32
+  leaf of every observation is exactly ``leaf.to(obs_dtype)`` of the fp32 one, rounded where the step already
+  writes or copies its results (no launch of its own); the scenario still computes in fp32;
 * ``cuda_graph=True`` captures one whole ``step`` (action decoding → dynamics → physics kernels →
   scenario reward / observation / done / info) into a CUDA graph after two eager warm-up steps
   and replays it afterwards: no Python, no per-kernel launch latency.  It requires a
@@ -103,6 +106,22 @@ def _seeded(method):
 _FORK_OBSERVATIONS = os.environ.get("VMAS_B200_FORK_OBS", "0") == "1"
 
 
+#: what ``Environment(obs_dtype=...)`` accepts
+OBS_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def check_obs_dtype(obs_dtype):
+    if obs_dtype not in OBS_DTYPES:
+        raise ValueError(f"obs_dtype must be torch.float32, torch.float16 or torch.bfloat16, not {obs_dtype!r}")
+
+
+def _to_obs_dtype(x, dtype):
+    """A fresh copy of one agent's observation with every fp32 leaf as ``dtype`` (other leaves cloned as they are)."""
+    if isinstance(x, Tensor):
+        return x.to(dtype) if x.dtype == torch.float32 else x.clone()
+    return {k: _to_obs_dtype(v, dtype) for k, v in x.items()}
+
+
 def _leaves(x):
     if isinstance(x, Tensor):
         yield x
@@ -134,8 +153,10 @@ class Environment(TorchVectorizedObject):
         action_checks: Optional[str] = None,
         cuda_graph: bool = False,
         auto_reset: bool = False,
+        obs_dtype: torch.dtype = torch.float32,
         **kwargs,
     ):
+        check_obs_dtype(obs_dtype)
         if multidiscrete_actions:
             assert (
                 not continuous_actions
@@ -170,6 +191,7 @@ class Environment(TorchVectorizedObject):
                 raise ValueError("cuda_graph=True needs a CUDA device")
             self.cuda_graph = cuda_graph
             self.auto_reset = auto_reset
+            self.obs_dtype = obs_dtype
             if auto_reset and not self.scenario.supports_masked_reset:
                 raise NotImplementedError(
                     f"auto_reset=True needs a scenario whose reset_world_at accepts a bool mask "
@@ -315,6 +337,10 @@ class Environment(TorchVectorizedObject):
         # graph mode clones once, outside the captured region, instead
         _c = (lambda t: t.clone()) if clone else (lambda t: t)
         _rc = TorchUtils.recursive_clone if clone else (lambda t: t)
+        # observations: the same clone, or the conversion to 16 bits in its place (graph mode: the hand-out copy)
+        _oc = _rc
+        if clone and self.obs_dtype != torch.float32:
+            _oc = lambda t: _to_obs_dtype(t, self.obs_dtype)  # noqa: E731
 
         def collect(fn):
             out = {} if by_name else []
@@ -345,11 +371,11 @@ class Environment(TorchVectorizedObject):
             side = self._obs_stream
             side.wait_stream(main)
             with torch.cuda.stream(side):
-                obs = collect(lambda a: _rc(self.scenario.observation(a)))
+                obs = collect(lambda a: _oc(self.scenario.observation(a)))
         # order matters: scenarios cache shared terms while computing agent 0's reward
         rewards = collect(lambda a: _c(self.scenario.reward(a))) if get_rewards else None
         if get_observations and not fork:
-            obs = collect(lambda a: _rc(self.scenario.observation(a)))
+            obs = collect(lambda a: _oc(self.scenario.observation(a)))
         infos = collect(lambda a: _rc(self.scenario.info(a))) if get_infos else None
         if self.terminated_truncated:
             terminated = truncated = None
@@ -663,7 +689,10 @@ class Environment(TorchVectorizedObject):
 
     def _pack_graph_outputs(self, outputs):
         """(inside the capture) lays the output leaves out as a few flat blocks — one per big contiguous
-        run, one per dtype for the small leaves — and prepares the copy that hands them out."""
+        run, one per dtype for the small leaves — and prepares the copy that hands them out.  With a 16-bit
+        ``obs_dtype`` the fp32 observation leaves (``outputs[0]``) get blocks of that type to themselves,
+        and the hand-out copy rounds them on the way."""
+        N = self.world._get_backend()._native
         leaves = []
 
         def index(x):
@@ -678,6 +707,8 @@ class Environment(TorchVectorizedObject):
 
         spec = index(outputs)
         index = None  # the recursive closure references itself: break the cycle
+        n_obs = len(list(_leaves(outputs[0]))) if self.obs_dtype != torch.float32 else 0
+        converted = [i < n_obs and t.dtype == torch.float32 for i, t in enumerate(leaves)]
         # Runs of leaves that already sit back to back in one allocation (e.g. the rows of a
         # batched [A, B, F] observation block) are handed out as ONE view.  A big run is its own
         # pack (cloned as is: no gather copy in the graph); the small rest is concatenated into
@@ -690,6 +721,7 @@ class Environment(TorchVectorizedObject):
                 if (
                     head.is_contiguous()
                     and head.dtype == t.dtype
+                    and converted[first] == converted[i]
                     and t.untyped_storage().data_ptr() == head.untyped_storage().data_ptr()
                     and t.data_ptr() == head.data_ptr() + numel * head.element_size()
                 ):
@@ -704,27 +736,35 @@ class Environment(TorchVectorizedObject):
             if head.is_contiguous() and numel * head.element_size() >= self.PACK_ALONE_BYTES:
                 packs.append((head.as_strided((numel,), (1,)), ids))
             else:
-                small.setdefault(head.dtype, []).extend(ids)
+                small.setdefault((head.dtype, converted[first]), []).extend(ids)
         # The small leaves of a dtype form one output block too, but nothing gathers them inside the graph:
         # the hand-out copy reads every leaf where the scenario wrote it (sources[i] = the pieces of block
         # i, in order).  A non-contiguous leaf is made contiguous by a copy node (rare: scenarios return
         # fresh or [B]-row tensors).
         sources = [[pack] for pack, _ in packs]
-        for dtype, ids in small.items():
+        for _, ids in small.items():
             pieces = [leaves[i] if leaves[i].is_contiguous() else leaves[i].contiguous() for i in ids]
             total = sum(t.numel() for t in pieces)
             packs.append((None, ids))
             sources.append([t.reshape(-1) for t in pieces])
-        self._graph_out_blocks = [(sum(t.numel() for t in pieces), pieces[0].dtype) for pieces in sources]
+        # per block: what the hand-out copy makes of its fp32 sources (DTYPE_F32: a plain copy)
+        kinds = [N.DTYPE_CODES[self.obs_dtype] if converted[ids[0]] else N.DTYPE_F32 for _, ids in packs]
+        self._graph_out_blocks = [
+            (sum(t.numel() for t in pieces), self.obs_dtype if kind else pieces[0].dtype)
+            for pieces, kind in zip(sources, kinds)
+        ]
+        self._graph_out_block_kinds = kinds
         items, copies_per_block = [], []
         for block, pieces in enumerate(sources):
             offset = 0
+            size = self._graph_out_blocks[block][1].itemsize
             for t in pieces:
                 if t.numel():
                     items.append((t, block, offset))
-                offset += t.numel() * t.element_size()
-        N = self.world._get_backend()._native
-        self._graph_out_copy = [N.CopyPlan(items[lo : lo + N.MAX_COPY_SEGMENTS]) for lo in range(0, len(items), N.MAX_COPY_SEGMENTS)]
+                offset += t.numel() * size
+        self._graph_out_copy = [
+            N.CopyPlan(items[lo : lo + N.MAX_COPY_SEGMENTS], kinds) for lo in range(0, len(items), N.MAX_COPY_SEGMENTS)
+        ]
         self._graph_out_spec = spec
         self._graph_out_shapes = [tuple(t.shape) for t in leaves]
         self._graph_out_packs = packs
@@ -878,6 +918,7 @@ class Environment(TorchVectorizedObject):
                 backend.lib, backend._dev_tables, self.world.slab, arr, len(live), self.clamp_action,
                 self._bad_action_flag if self.action_checks == "deferred" else None, self.steps if counts else None,
                 ingest_built_mask, graph.raw_cuda_graph_exec(), items, len(self._graph_out_blocks),
+                block_kinds=self._graph_out_block_kinds,
             )
         else:
             mode, c, prog, oplan, cols, out = direct
@@ -887,13 +928,18 @@ class Environment(TorchVectorizedObject):
                 # results the post stage can write straight into the step's fresh blocks instead of into static
                 # buffers that are then copied: the observation rows (if one leaf run covers the whole block),
                 # and every leaf that is an output of the program (one more STORE per leaf)
-                c, instrs, items, obs_to, mirrors = self._results_in_place(c, prog, instrs, items, cols, out)
+                c, instrs, items, obs_to, mirrors = self._results_in_place(
+                    c, prog, instrs, items, cols, out, self._graph_out_block_kinds
+                )
+            # the post stage rounds the observation rows itself where it writes them into the fresh block
+            obs_dtype = N.DTYPE_F32 if obs_to is None else self._graph_out_block_kinds[obs_to[0]]
             plan = N.EnvStepPlan(
                 backend.lib, backend._dev_tables, self.world.slab, arr, len(live), self.clamp_action,
                 self._bad_action_flag if self.action_checks == "deferred" else None, self.steps if counts else None,
                 ingest_built_mask, 0, items, len(self._graph_out_blocks), program=c, columns=cols,
                 n_rows=0 if oplan is None else oplan.n_rows, width=0 if oplan is None else oplan.width, obs_out=out,
-                exact_broad_phase=mode, obs_to=obs_to, mirrors=mirrors,
+                exact_broad_phase=mode, obs_to=obs_to, mirrors=mirrors, block_kinds=self._graph_out_block_kinds,
+                obs_dtype=obs_dtype,
             )
             plan.keep += (prog, oplan)
             if _WHOLE_STEP_KERNEL and backend._dev_tables.tb.specialization >= 0:
@@ -921,7 +967,7 @@ class Environment(TorchVectorizedObject):
                         for c in arr
                     )
                     plan.c.ingest_in_kernel = 1
-                job = jit.request_step_kernel(backend.tables.desc, cols_np, instrs, acts)
+                job = jit.request_step_kernel(backend.tables.desc, cols_np, instrs, acts, obs_dtype=obs_dtype)
                 if job is not None:
                     job.done.wait(timeout=_WHOLE_STEP_KERNEL_WAIT_S)
         if direct is not None and direct[3] is not None and direct[3].buffer_sources and not (
@@ -938,9 +984,11 @@ class Environment(TorchVectorizedObject):
         self._adopt_whole_step_kernel(plan)
         return plan
 
-    def _results_in_place(self, c, prog, instrs, items, cols, out):
+    def _results_in_place(self, c, prog, instrs, items, cols, out, block_kinds=None):
         """Splits the hand-out copies ``items`` = [(source, block, byte offset)] into what the post stage can
-        write in place.  Returns ``(program struct with the extra stores, its instructions, the copies that
+        write in place.  ``block_kinds[b]``: ``DTYPE_F16`` / ``DTYPE_BF16`` if block ``b`` receives its fp32
+        sources rounded to 16 bits (the observation rows are then written in place as such; no program store is
+        mirrored into it).  Returns ``(program struct with the extra stores, its instructions, the copies that
         remain, (block, offset) of the observation rows or None, [(buffer slot, block, offset)])``."""
         from ... import _native as N
         from .. import program as SP
@@ -962,10 +1010,11 @@ class Environment(TorchVectorizedObject):
             inside = [k for k, (src, _, _) in enumerate(items) if lo <= src.data_ptr() < lo + size]
             if inside:
                 _, block0, offset0 = items[inside[0]]
+                shrink = 2 if block_kinds and block_kinds[block0] else 1  # (fp32 rows land as 16-bit values)
                 at = 0
                 for k in inside:
                     src, block, offset = items[k]
-                    if src.data_ptr() != lo + at or block != block0 or offset != offset0 + at:
+                    if src.data_ptr() != lo + at or block != block0 or offset != offset0 + at // shrink:
                         break
                     at += src.numel() * src.element_size()
                 else:
@@ -976,7 +1025,7 @@ class Environment(TorchVectorizedObject):
                 continue
             o = by_ptr.get((src.data_ptr(), src.dtype))
             if (
-                o is not None and src.numel() == B and o._slot in store_of
+                o is not None and src.numel() == B and o._slot in store_of and not (block_kinds and block_kinds[block])
                 and n_slots + len(extra) < N.PROG_MAX_BUFFERS and len(instrs) + len(extra) < N.PROG_MAX_INSTR
             ):
                 op, reg = store_of[o._slot]
@@ -1090,9 +1139,9 @@ class Environment(TorchVectorizedObject):
 
     def get_agent_observation_space(self, agent: Agent, obs: AGENT_OBS_TYPE):
         if isinstance(obs, Tensor):
-            return spaces.Box(
-                low=-np.float32("inf"), high=np.float32("inf"), shape=obs.shape[1:], dtype=np.float32
-            )
+            # obs_dtype=torch.bfloat16: numpy has no bfloat16, the space stays fp32
+            dtype = np.float16 if self.obs_dtype == torch.float16 else np.float32
+            return spaces.Box(low=-dtype("inf"), high=dtype("inf"), shape=obs.shape[1:], dtype=dtype)
         if isinstance(obs, Dict):
             return spaces.Dict(
                 {k: self.get_agent_observation_space(agent, v) for k, v in obs.items()}
