@@ -151,12 +151,13 @@ def emit_world(desc: P.WorldDescription, label: str, tuning: Dict = None) -> Tup
 def post_hash(cols, instrs, acts=(), obs_dtype: int = 0) -> int:
     """FNV-1a 64 of what a whole-step kernel does around the substeps: the observation plan's column table
     (int32 ``[rows, width, 4]`` or None), the step program's instructions ``[(op, dst, a, b, arg, imm)]`` with
-    entity indices resolved, the action ingest ``[(agent row, u_range x 2, u_multiplier x 2)]`` of the
-    policy agents (empty: actions are ingested by a launch of their own) and the type of the observation rows
-    (``VMAS_DTYPE_*``; fp32 adds nothing to the hash)."""
+    entity indices resolved, the action ingest ``[(agent row, u_range x 2, u_multiplier x 2[, kind, nvec x 2])]``
+    of the policy agents (empty: actions are ingested by a launch of their own; the last three for discrete and
+    multi-discrete spaces only, ``VMAS_ACT_*``) and the type of the observation rows (``VMAS_DTYPE_*``; fp32 adds
+    nothing to the hash)."""
     parts = [None if cols is None else [list(cols.shape), [int(x) for x in cols.reshape(-1)]],
              [[int(op), int(dst), int(a), int(b), int(arg), _f(imm)] for op, dst, a, b, arg, imm in instrs],
-             [[int(agent)] + [_f(v) for v in rest] for agent, *rest in acts]]
+             [[int(act[0])] + [_f(v) for v in act[1:5]] + [int(v) for v in act[5:]] for act in acts]]
     if obs_dtype:
         parts.append(int(obs_dtype))
     blob = json.dumps(parts).encode()
@@ -195,8 +196,9 @@ def emit_post(cols, instrs, acts=(), obs_dtype: int = 0) -> Tuple[str, str, int]
         f"OBS_DTYPE = {int(obs_dtype)};"
     )
     lines.append(f"  static constexpr ActC act[{max(len(acts), 1)}] = {{")
-    for agent, r0, r1, m0, m1 in acts:
-        lines.append(f"      {{{int(agent)}, {_f(r0)}, {_f(r1)}, {_f(m0)}, {_f(m1)}}},")
+    for agent, r0, r1, m0, m1, *discrete in acts:
+        tail = "".join(f", {int(v)}" for v in discrete)  # (kind, n0, n1: continuous agents keep the defaults)
+        lines.append(f"      {{{int(agent)}, {_f(r0)}, {_f(r1)}, {_f(m0)}, {_f(m1)}{tail}}},")
     if not acts:
         lines.append("      {0, 0.f, 0.f, 0.f, 0.f},")
     lines.append("  };")

@@ -37,6 +37,21 @@ DEVI float ingest_continuous(float v, const float r, const float m, const bool c
   return v * m;
 }
 
+// One discrete action component (ref environment.py:656-706): index k of n choices becomes one of n evenly
+// spaced values in [-r, r], scaled by m.  For odd n index 0 means "no force" and indices 1 .. n/2 shift down by
+// one.  An index outside [0, n) sets `bad` and still decodes by the same formula.  (index, r and m by reference:
+// then nvcc compiles ingest_actions_body to the same instructions as with this code written in line there.)
+DEVI float ingest_discrete(const long long& index, const long long n, const float& r, const float& m, bool& bad) {
+  long long k = index;
+  bad |= k < 0 || k >= n;
+  if (n % 2 != 0) {
+    if (k == 0) k = n / 2;
+    else if (k <= n / 2) k = k - 1;
+  }
+  const float v = ((float)k / (float)(n - 1)) * (2.f * r) - r;
+  return v * m;
+}
+
 // ---- the kinematic action models (ref dynamics/diff_drive.py, kinematic_bicycle.py, drone.py) ---------
 // Each integrates a small ODE over dt — classic RK4 or Euler, the reference's order of operations — to
 // get the pose change the command asks for.
@@ -135,14 +150,7 @@ DEVI void ingest_actions_body(const IngestArgs& a, const long idx) {
         } else {
           k = idx_in[env * sz + j];
         }
-        bad |= k < 0 || k >= n;
-        if (n % 2 != 0) {  // odd n: index 0 means "no force"; indices 1 .. n/2 shift down by one
-          if (k == 0) k = n / 2;
-          else if (k <= n / 2) k = k - 1;
-        }
-        const float r = ag.u_range[j];
-        const float v = ((float)k / (float)(n - 1)) * (2.f * r) - r;
-        u[j] = v * ag.u_multiplier[j];
+        u[j] = ingest_discrete(k, n, ag.u_range[j], ag.u_multiplier[j], bad);
       }
     }
   }

@@ -53,17 +53,24 @@ struct EpiArgs {
   void* obs_out;  // [rows, B, width] of P::OBS_DTYPE (fp32, fp16 or bf16), or null
   void* buffers[VMAS_PROG_MAX_BUFFERS];
 };
-// ... and its prologue (see spec_ingest): the policy agents' continuous holonomic actions
+// ... and its prologue (see spec_ingest_lane): the policy agents' holonomic actions, continuous, discrete or
+// multi-discrete
 struct ActC {
   int agent;  // row of the agent in the force / torque slab
   float range0, range1, mult0, mult1;
+  int kind = VMAS_ACT_CONTINUOUS;  // VMAS_ACT_*
+  int n0 = 0, n1 = 0;              // (discrete kinds) choices per component
 };
 struct ActArgs {
-  const float* actions[VMAS_MAX_INGEST_AGENTS];  // [B, 2] each, the caller's tensors
+  const float* actions[VMAS_MAX_INGEST_AGENTS];  // the caller's tensors: fp32 [B, 2], or int64 [B, 1] / [B, 2]
   float* u[VMAS_MAX_INGEST_AGENTS];              // [B, 2] each: agent.action.u
   uint8_t* bad_flag;
   float* steps;  // [B] or null
   int clamp;
+  int kind[VMAS_MAX_INGEST_AGENTS];  // VMAS_ACT_* of each agent's tensor: launch_env refuses one it was not built for
+};
+struct alignas(16) ActIdx2 {  // one multi-discrete env row, loaded as one 16-byte word
+  long long i0, i1;
 };
 
 struct SpecArgs {
@@ -1066,6 +1073,65 @@ DEVI void spec_env_step(const SpecArgs& a, const long env, const uint32_t (&mask
   }
 }
 
+// ---- the action prologue of the one-kernel step (step_env_kernel), one lane at a time ----------------------------
+// Round J of G lanes per env: agent k0 = G J on the even lane, k1 = G J + G - 1 on the odd lane (k1 = k0 for a lone
+// agent or G = 1: both lanes decode it).
+template <class P, int G, int J>
+struct SpecActRound {
+  static constexpr int k0 = J * G, k1 = k0 + G - 1 < P::N_ACT ? k0 + G - 1 : k0;
+};
+
+// The lane's agent's action, decoded as the ingest kernel does (ingest_continuous / ingest_discrete; a discrete
+// flat index is unravelled by the same truncating / and %), stored to agent.action.u (live envs; a lone agent's
+// from the even lane) and returned.  `bad` collects the flag.  No clamp for discrete kinds.
+template <class P, int G, int J>
+DEVI float2 spec_ingest_lane(const ActArgs& act, const long env, const bool odd, const bool live, bool& bad) {
+  constexpr int k0 = SpecActRound<P, G, J>::k0, k1 = SpecActRound<P, G, J>::k1;
+  constexpr ActC c0 = P::act[k0], c1 = P::act[k1];
+  static_assert(c0.kind == c1.kind, "one action kind per round");
+  const bool o = k0 != k1 && odd;
+  const float range0 = o ? c1.range0 : c0.range0, range1 = o ? c1.range1 : c0.range1;
+  float2 u;
+  if constexpr (c0.kind == VMAS_ACT_CONTINUOUS) {
+    const float2 v = reinterpret_cast<const float2*>(o ? act.actions[k1] : act.actions[k0])[env];
+    const float ux = ingest_continuous(v.x, range0, o ? c1.mult0 : c0.mult0, act.clamp, bad);
+    u = make_float2(ux, ingest_continuous(v.y, range1, o ? c1.mult1 : c0.mult1, act.clamp, bad));
+  } else {
+    const void* in = o ? act.actions[k1] : act.actions[k0];
+    const long long n1 = o ? c1.n1 : c0.n1;
+    long long i0, i1;
+    if constexpr (c0.kind == VMAS_ACT_DISCRETE) {  // [B, 1]: the flat index of the product of the two components
+      const long long flat = static_cast<const long long*>(in)[env];
+      i0 = flat / n1;
+      i1 = flat % n1;
+    } else {  // [B, 2]
+      const ActIdx2 k = static_cast<const ActIdx2*>(in)[env];
+      i0 = k.i0;
+      i1 = k.i1;
+    }
+    const float ux = ingest_discrete(i0, o ? c1.n0 : c0.n0, range0, o ? c1.mult0 : c0.mult0, bad);
+    u = make_float2(ux, ingest_discrete(i1, n1, range1, o ? c1.mult1 : c0.mult1, bad));
+  }
+  if (live && (k0 != k1 || !odd)) reinterpret_cast<float2*>(o ? act.u[k1] : act.u[k0])[env] = u;
+  return u;
+}
+
+// ... and round J's force rows on the lane: its own u, and p = the partner lane's u (a pair of agents only)
+template <class P, int G, int J>
+DEVI void spec_ingest_put(const float2 u, const float2 p, const bool odd, float* afx, float* afy) {
+  constexpr int k0 = SpecActRound<P, G, J>::k0, k1 = SpecActRound<P, G, J>::k1;
+  constexpr ActC c0 = P::act[k0], c1 = P::act[k1];
+  if constexpr (k0 == k1) {
+    afx[c0.agent] = u.x;
+    afy[c0.agent] = u.y;
+  } else {
+    afx[c0.agent] = odd ? p.x : u.x;
+    afy[c0.agent] = odd ? p.y : u.y;
+    afx[c1.agent] = odd ? u.x : p.x;
+    afy[c1.agent] = odd ? u.y : p.y;
+  }
+}
+
 #ifdef __CUDACC__
 // SCHED: the env-scheduling variant (thread t steps env order[t], signatures recorded); the default
 // kernel carries none of that code
@@ -1134,8 +1200,8 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_fused_kernel(con
 
 // ---- the whole Environment.step as ONE kernel -----------------------------------------------------------
 // step_fused_kernel plus what the ingest launch in front of it does (vmas_b200_ingest_actions_broad_phase):
-// every thread decodes its env's actions (continuous, holonomic: ref environment.py:616-655, 707 and
-// dynamics/holonomic.py:14-15) straight into the force registers, counts the step, and tests its env's
+// every thread decodes its env's actions (holonomic; continuous, discrete or multi-discrete: ref
+// environment.py:616-707 and dynamics/holonomic.py:14-15) straight into the force registers, counts the step, and tests its env's
 // masked pairs for the batch-wide broad phase (ref core.py:2797-2801); the mask is complete once every block
 // has contributed — a grid-wide barrier, which needs all blocks resident (cooperative launch; the launcher
 // says no for batches beyond that and the caller keeps the separate ingest launch).
@@ -1219,24 +1285,12 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
   // the actions: agents k0 = G j and k1 = G j + G - 1 on the lanes of a pair
   bool bad = false;
   static_for<(P::N_ACT + G - 1) / G>([&](auto ji) {
-    constexpr int k0 = decltype(ji)::value * G, k1 = k0 + G - 1 < P::N_ACT ? k0 + G - 1 : k0;
-    constexpr ActC c0 = P::act[k0], c1 = P::act[k1];
-    const bool o = k0 != k1 && odd;
-    const float range0 = o ? c1.range0 : c0.range0, range1 = o ? c1.range1 : c0.range1;
-    const float2 v = reinterpret_cast<const float2*>(o ? act.actions[k1] : act.actions[k0])[env];
-    const float ux = ingest_continuous(v.x, range0, o ? c1.mult0 : c0.mult0, act.clamp, bad);
-    const float2 u = make_float2(ux, ingest_continuous(v.y, range1, o ? c1.mult1 : c0.mult1, act.clamp, bad));
-    if (live && (k0 != k1 || !odd)) reinterpret_cast<float2*>(o ? act.u[k1] : act.u[k0])[env] = u;
-    if constexpr (k0 == k1) {
-      afx[c0.agent] = u.x;
-      afy[c0.agent] = u.y;
-    } else {
-      const float2 p = make_float2(pair_swap(u.x), pair_swap(u.y));
-      afx[c0.agent] = odd ? p.x : u.x;
-      afy[c0.agent] = odd ? p.y : u.y;
-      afx[c1.agent] = odd ? u.x : p.x;
-      afy[c1.agent] = odd ? u.y : p.y;
-    }
+    constexpr int J = decltype(ji)::value;
+    const float2 u = spec_ingest_lane<P, G, J>(act, env, odd, live, bad);
+    if constexpr (SpecActRound<P, G, J>::k0 == SpecActRound<P, G, J>::k1)
+      spec_ingest_put<P, G, J>(u, u, odd, afx, afy);
+    else
+      spec_ingest_put<P, G, J>(u, make_float2(pair_swap(u.x), pair_swap(u.y)), odd, afx, afy);
   });
   if constexpr (G > 1) bad = __shfl_xor_sync(0xffffffffu, (int)bad, 1) || bad;
   if (live && !odd) {
@@ -1377,6 +1431,8 @@ static cudaError_t launch_env_lanes(const SpecArgs& a, const EpiArgs& e, const A
 // at once even so (masked worlds only)
 template <class W, class P>
 static cudaError_t launch_env(const SpecArgs& a, const EpiArgs& e, const ActArgs& act, cudaStream_t stream) {
+  for (int k = 0; k < P::N_ACT; ++k)  // (the kernel reads each agent's tensor as the kind it was compiled for)
+    if (act.kind[k] != P::act[k].kind) return cudaErrorInvalidValue;
   const long blocks = ((long)a.batch_dim + W::BLOCK - 1) / W::BLOCK;
   const bool coop = W::MASK_WORDS > 0 && a.use_mask;
   long cap = 0;

@@ -230,7 +230,8 @@ def request_step_kernel(desc: P.WorldDescription, cols, instrs, acts=(), block: 
     """Starts (or finds) the compilation of the whole-step kernel; None if the world cannot be specialised or
     has per-env physical parameters (those step on the captured graph of the specialised substep kernel).
     ``acts``: [(agent row, u_range x 2, u_multiplier x 2)] of the policy agents if the kernel is to ingest
-    their (continuous, holonomic) actions itself.  ``obs_dtype``: the type the kernel stores its observation
+    their (holonomic) actions itself; discrete and multi-discrete agents append (``VMAS_ACT_*`` kind, nvec x 2).
+    ``prebuild_step_kernels`` compiles the continuous variants only.  ``obs_dtype``: the type the kernel stores its observation
     rows as (``VMAS_DTYPE_*``; part of the key)."""
     if not available() or not codegen.specializable(desc):
         return None

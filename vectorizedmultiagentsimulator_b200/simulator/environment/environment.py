@@ -51,7 +51,8 @@ _DIRECT_STEP = os.environ.get("VMAS_B200_DIRECT_STEP", "1") != "0"
 _WHOLE_STEP_KERNEL = os.environ.get("VMAS_B200_WHOLE_STEP_KERNEL", "1") != "0"
 #: ... and writes the step's results straight into the fresh output blocks (no hand-out copy)
 _WRITE_RESULTS_IN_PLACE = os.environ.get("VMAS_B200_RESULTS_IN_PLACE", "1") != "0"
-#: ... with the action ingest and the broad phase inside that kernel too (continuous holonomic agents)
+#: ... with the action ingest and the broad phase inside that kernel too (holonomic agents; continuous, discrete or
+#: multi-discrete actions)
 _INGEST_IN_KERNEL = os.environ.get("VMAS_B200_INGEST_IN_KERNEL", "1") != "0"
 _WHOLE_STEP_KERNEL_WAIT_S = float(os.environ.get("VMAS_B200_WHOLE_STEP_KERNEL_WAIT_S", "60"))
 
@@ -953,10 +954,10 @@ class Environment(TorchVectorizedObject):
 
                     cols_np = codegen.fuse_value_columns(cols_np, oplan.buffer_sources, instrs)
                 # ... with the action ingest (and the broad phase) as its prologue where the agents allow it:
-                # the whole step is then ONE launch
+                # the whole step is then ONE launch.  Continuous, discrete and multi-discrete spaces alike.
                 acts = ()
                 if (
-                    _INGEST_IN_KERNEL and self.continuous_actions and len(live) == len(specs)
+                    _INGEST_IN_KERNEL and len(live) == len(specs)
                     and all(s[1] == N.DYN_HOLONOMIC and s[0].action_size == 2 for s in specs)
                     and type(self.scenario).pre_step is BaseScenario.pre_step and not self.world.scripted_agents
                     and (ingest_built_mask or backend.tables.n_masked == 0 or not self.world.exact_broad_phase)
@@ -964,6 +965,7 @@ class Environment(TorchVectorizedObject):
                     acts = tuple(
                         (int(c.agent_index), float(c.u_range[0]), float(c.u_range[1]), float(c.u_multiplier[0]),
                          float(c.u_multiplier[1]))
+                        + (() if self.continuous_actions else (int(c.action_kind), int(c.nvec[0]), int(c.nvec[1])))
                         for c in arr
                     )
                     plan.c.ingest_in_kernel = 1
@@ -979,6 +981,7 @@ class Environment(TorchVectorizedObject):
         plan.direct = direct is not None
         plan.job = job
         plan.live = live
+        plan.bind = [(agent.action, u) for agent, _, u in specs]
         plan.counts = counts
         plan.drones = list(getattr(backend, "_ingest_drones", []))
         self._adopt_whole_step_kernel(plan)
@@ -1073,6 +1076,9 @@ class Environment(TorchVectorizedObject):
         for j, c in enumerate(copies):
             blocks[j] = c.data_ptr()
         launched = plan.run()  # (the kernels the call issued itself; a graph's nodes come on top)
+        for action, u in plan.bind:  # (a reset replaces agent.action.u; the call writes the static buffers)
+            if action._u is not u:
+                action.u = u
         self.graph_replays += 1
         backend = self.world._get_backend()
         backend.launches += launched + (0 if plan.direct else self._graph_launches)
