@@ -16,6 +16,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 import torch
 from torch import Tensor
 
+from . import codegen
 from .simulator import plan as P
 
 
@@ -492,16 +493,10 @@ class CudaBackend(PlanRuntime):
                     for j, choices in enumerate(agent.discrete_action_nvec):
                         c.nvec[j] = int(choices)
                 if dyn >= self._native.DYN_DIFF_DRIVE:  # the kinematic models' parameters
-                    model = agent.dynamics
-                    params = [float(model.dt), float(agent.mass), float(agent.moment_of_inertia),
-                              1.0 if model.integration == "rk4" else 0.0, 0.0, 0.0, 0.0, 0.0]
-                    if dyn == self._native.DYN_BICYCLE:
-                        params[4:7] = [float(model.l_f), float(model.l_r), float(model.max_steering_angle)]
-                    elif dyn == self._native.DYN_DRONE:
-                        params[4:8] = [float(model.I_xx), float(model.I_yy), float(model.I_zz), float(model.g)]
-                        self._ingest_drones.append((c, model))
-                    for j, v in enumerate(params):
+                    for j, v in enumerate(codegen.dynamics_params(agent, dyn)):
                         c.dyn_params[j] = v
+                    if dyn == self._native.DYN_DRONE:
+                        self._ingest_drones.append((c, agent.dynamics))
                 rng = agent.action.u_range_tensor.tolist()
                 mul = agent.action.u_multiplier_tensor.tolist()
                 for j in range(agent.action_size):

@@ -17,6 +17,7 @@ from typing import Dict, List, Tuple
 
 import numpy as np
 
+from . import _native as N
 from .simulator import plan as P
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -148,16 +149,92 @@ def emit_world(desc: P.WorldDescription, label: str, tuning: Dict = None) -> Tup
     return name, "\n".join(lines), h
 
 
+# ---- the action prologue of the one-kernel step -------------------------------------------------------------------
+#: the action models the prologue runs (``VMAS_DYN_*``: holonomic, holonomic with rotation, forward, rotation,
+#: differential drive) and the action size each takes: the model's own.  Left to the ingest launch: the kinematic
+#: bicycle (its prologue measured slower than its two-launch step on the H100, DESIGN §7.4) and the drone (a 12-state
+#: RK4 per agent).
+PROLOGUE_MODELS = {N.DYN_HOLONOMIC: 2, N.DYN_HOLONOMIC_ROT: 3, N.DYN_FORWARD: 1, N.DYN_ROTATION: 1,
+                   N.DYN_DIFF_DRIVE: 2}
+
+
+def dynamics_code(dynamics):
+    """``VMAS_DYN_*`` of an agent's dynamics model (exact types: a subclass may override ``process_action``), or
+    None if the ingest kernel does not implement it."""
+    from .simulator.dynamics.basic import Forward, Holonomic, HolonomicWithRotation, Rotation, Static
+    from .simulator.dynamics.diff_drive import DiffDrive
+    from .simulator.dynamics.drone import Drone
+    from .simulator.dynamics.kinematic_bicycle import KinematicBicycle
+
+    return {
+        Holonomic: N.DYN_HOLONOMIC, HolonomicWithRotation: N.DYN_HOLONOMIC_ROT, Forward: N.DYN_FORWARD,
+        Rotation: N.DYN_ROTATION, Static: N.DYN_NONE, DiffDrive: N.DYN_DIFF_DRIVE, KinematicBicycle: N.DYN_BICYCLE,
+        Drone: N.DYN_DRONE,
+    }.get(type(dynamics))
+
+
+def dynamics_params(agent, dyn: int) -> List[float]:
+    """``VmasAgentActions::dyn_params`` of a kinematic model: dt, mass, moment of inertia, rk4 (1 / 0), then the
+    bicycle's l_f, l_r, max steering angle or the drone's I_xx, I_yy, I_zz, g.  Zeros for the other models."""
+    params = [0.0] * 8
+    if dyn >= N.DYN_DIFF_DRIVE:
+        model = agent.dynamics
+        params[:4] = [float(model.dt), float(agent.mass), float(agent.moment_of_inertia),
+                      1.0 if model.integration == "rk4" else 0.0]
+        if dyn == N.DYN_BICYCLE:
+            params[4:7] = [float(model.l_f), float(model.l_r), float(model.max_steering_angle)]
+        elif dyn == N.DYN_DRONE:
+            params[4:8] = [float(model.I_xx), float(model.I_yy), float(model.I_zz), float(model.g)]
+    return params
+
+
+def prologue_acts(agents, kind: int = N.ACT_CONTINUOUS) -> tuple:
+    """The ``acts`` of a whole-step kernel whose prologue ingests the actions of ``agents`` (the policy agents with
+    action components, in ingest order; each with the fields of ``VmasAgentActions``: ``agent_index``,
+    ``dynamics``, ``action_size``, ``u_range``, ``u_multiplier``, ``nvec``, ``dyn_params``), or ``()`` if the
+    prologue does not take them all: every agent's model must be in ``PROLOGUE_MODELS`` with its own action size,
+    and there are at most ``VMAS_MAX_INGEST_AGENTS``.  ``kind``: ``VMAS_ACT_*`` of the action space.
+
+    An entry is ``(agent row, u_range x 2, u_multiplier x 2)`` for a holonomic agent with 2 components and continuous
+    actions, plus ``(kind, nvec x 2)`` for discrete ones: the text and the key of those kernels stay what they were
+    before the other models.  Other agents: ``(row, u_range x 2, u_multiplier x 2, kind, nvec x 2, dynamics, size,
+    u_range[2:4], u_multiplier[2:4], nvec[2:4], dyn_params x 8)`` (``ActC`` in csrc/spec_kernel.cuh)."""
+    if not agents or len(agents) > N.MAX_INGEST_AGENTS:
+        return ()
+    acts = []
+    for c in agents:
+        dyn, size = int(c.dynamics), int(c.action_size)
+        if PROLOGUE_MODELS.get(dyn) != size:
+            return ()
+        rng = [float(c.u_range[j]) if j < size else 0.0 for j in range(4)]
+        mul = [float(c.u_multiplier[j]) if j < size else 0.0 for j in range(4)]
+        nvec = [int(c.nvec[j]) if kind != N.ACT_CONTINUOUS and j < size else 0 for j in range(4)]
+        act = (int(c.agent_index), rng[0], rng[1], mul[0], mul[1])
+        if dyn == N.DYN_HOLONOMIC and size == 2:
+            acts.append(act + (() if kind == N.ACT_CONTINUOUS else (int(kind), nvec[0], nvec[1])))
+        else:
+            acts.append(act + (int(kind), nvec[0], nvec[1], dyn, size, rng[2], rng[3], mul[2], mul[3], nvec[2],
+                               nvec[3]) + tuple(float(c.dyn_params[j]) for j in range(8)))
+    return tuple(acts)
+
+
+def _act_fields(act) -> list:
+    """One ``acts`` entry as the typed list the key hashes (see ``prologue_acts``)."""
+    fields = [int(act[0])] + [_f(v) for v in act[1:5]] + [int(v) for v in act[5:10]]
+    if len(act) > 10:
+        fields += [_f(v) for v in act[10:14]] + [int(v) for v in act[14:16]] + [_f(v) for v in act[16:]]
+    return fields
+
+
 def post_hash(cols, instrs, acts=(), obs_dtype: int = 0) -> int:
     """FNV-1a 64 of what a whole-step kernel does around the substeps: the observation plan's column table
     (int32 ``[rows, width, 4]`` or None), the step program's instructions ``[(op, dst, a, b, arg, imm)]`` with
-    entity indices resolved, the action ingest ``[(agent row, u_range x 2, u_multiplier x 2[, kind, nvec x 2])]``
-    of the policy agents (empty: actions are ingested by a launch of their own; the last three for discrete and
-    multi-discrete spaces only, ``VMAS_ACT_*``) and the type of the observation rows (``VMAS_DTYPE_*``; fp32 adds
-    nothing to the hash)."""
+    entity indices resolved, the action ingest of the policy agents (``prologue_acts``; empty: actions are ingested
+    by a launch of their own) and the type of the observation rows (``VMAS_DTYPE_*``; fp32 adds nothing to the
+    hash)."""
     parts = [None if cols is None else [list(cols.shape), [int(x) for x in cols.reshape(-1)]],
              [[int(op), int(dst), int(a), int(b), int(arg), _f(imm)] for op, dst, a, b, arg, imm in instrs],
-             [[int(act[0])] + [_f(v) for v in act[1:5]] + [int(v) for v in act[5:]] for act in acts]]
+             [_act_fields(act) for act in acts]]
     if obs_dtype:
         parts.append(int(obs_dtype))
     blob = json.dumps(parts).encode()
@@ -196,8 +273,12 @@ def emit_post(cols, instrs, acts=(), obs_dtype: int = 0) -> Tuple[str, str, int]
         f"OBS_DTYPE = {int(obs_dtype)};"
     )
     lines.append(f"  static constexpr ActC act[{max(len(acts), 1)}] = {{")
-    for agent, r0, r1, m0, m1, *discrete in acts:
-        tail = "".join(f", {int(v)}" for v in discrete)  # (kind, n0, n1: continuous agents keep the defaults)
+    for act in acts:
+        agent, r0, r1, m0, m1 = act[:5]
+        tail = "".join(f", {int(v)}" for v in act[5:10])  # (kind, n0, n1[, dyn, size]: else the defaults)
+        if len(act) > 10:
+            tail += "".join(f", {_f(v)}" for v in act[10:14]) + "".join(f", {int(v)}" for v in act[14:16])
+            tail += ", {" + ", ".join(_f(v) for v in act[16:]) + "}"
         lines.append(f"      {{{int(agent)}, {_f(r0)}, {_f(r1)}, {_f(m0)}, {_f(m1)}{tail}}},")
     if not acts:
         lines.append("      {0, 0.f, 0.f, 0.f, 0.f},")

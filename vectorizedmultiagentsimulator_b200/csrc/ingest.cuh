@@ -114,6 +114,46 @@ DEVI Drone12 drone_f(const Drone12& s, float thrust, float tx, float ty, float t
   return d;
 }
 
+// ---- the action models: force / torque from the decoded action u (ref dynamics/*.py) ---------------------------
+// ingest_actions_body and the prologue of the one-kernel step (spec_kernel.cuh, spec_act_agent) both call these.
+// (The drone's 12-state RK4 stays in ingest_actions_body: the prologue leaves drones to the ingest launch, and
+// bicycles too: codegen.PROLOGUE_MODELS.)
+// What each model writes into the slab: the agent's force row, its torque row
+__host__ __device__ constexpr bool dyn_writes_force(int dyn) {
+  return dyn == VMAS_DYN_HOLONOMIC || dyn == VMAS_DYN_HOLONOMIC_ROT || dyn == VMAS_DYN_FORWARD || dyn >= VMAS_DYN_DIFF_DRIVE;
+}
+__host__ __device__ constexpr bool dyn_writes_torque(int dyn) {
+  return dyn == VMAS_DYN_HOLONOMIC_ROT || dyn == VMAS_DYN_ROTATION || dyn >= VMAS_DYN_DIFF_DRIVE;
+}
+
+// Forward: (u0, 0) rotated by the heading (ref dynamics/forward.py)
+DEVI float2 forward_force(const float u0, const float rot) {
+  float s, c;
+  sincosf(rot, &s, &c);
+  return make_float2(u0 * c - 0.f * s, u0 * s + 0.f * c);
+}
+
+// DiffDrive: the pose change of (v, w) = (u0, u1) over dt
+DEVI Pose3 diff_drive_pose(const float v, const float w, const float yaw, const float dt, const bool rk4) {
+  return integrate_pose(yaw, dt, rk4, [&](float h) { return diff_drive_f(h, v, w); });
+}
+
+// KinematicBicycle: the pose change of (v, steering) = (u0, u1) over dt, the steering clamped to +-lim
+DEVI Pose3 bicycle_pose(const float v, const float steering, const float yaw, const float dt, const bool rk4,
+                        const float l_f, const float l_r, const float lim) {
+  const float steer = fminf(fmaxf(steering, -lim), lim);
+  return integrate_pose(yaw, dt, rk4, [&](float h) { return bicycle_f(h, steer, v, l_f, l_r); });
+}
+
+// the force / torque that realise a kinematic model's pose change under the world's integrator (dynamics/common)
+DEVI float2 kinematic_force(const Pose3& d, const float dt, const float mass, const float inertia, const float2 vel,
+                            const float w0, float& torque) {
+  const float dt2 = dt * dt;
+  const float2 f = make_float2(mass * ((d.x - vel.x * dt) / dt2), mass * ((d.y - vel.y * dt) / dt2));
+  torque = inertia * ((d.yaw - w0 * dt) / dt2);
+  return f;
+}
+
 // KIN: the launch has an agent with a kinematic model (diff drive / bicycle / drone); the lean
 // instantiation without that code needs half the registers, and most scenarios use it
 template <bool KIN>
@@ -169,10 +209,8 @@ DEVI void ingest_actions_body(const IngestArgs& a, const long idx) {
       torque = u[2];
       write_torque = true;
     }
-  } else if (dyn == VMAS_DYN_FORWARD) {  // (u0, 0) rotated by the heading (ref dynamics/forward.py)
-    float s, c;
-    sincosf(a.st.rot[ent], &s, &c);
-    force = make_float2(u[0] * c - 0.f * s, u[0] * s + 0.f * c);
+  } else if (dyn == VMAS_DYN_FORWARD) {
+    force = forward_force(u[0], a.st.rot[ent]);
     write_force = true;
   } else if (dyn == VMAS_DYN_ROTATION) {
     torque = u[0];
@@ -183,12 +221,9 @@ DEVI void ingest_actions_body(const IngestArgs& a, const long idx) {
     const float yaw = a.st.rot[ent];
     Pose3 d;
     if (dyn == VMAS_DYN_DIFF_DRIVE) {
-      const float v = u[0], w = u[1];
-      d = integrate_pose(yaw, dt, rk4, [&](float h) { return diff_drive_f(h, v, w); });
+      d = diff_drive_pose(u[0], u[1], yaw, dt, rk4);
     } else if (dyn == VMAS_DYN_BICYCLE) {
-      const float l_f = ag.dyn_params[4], l_r = ag.dyn_params[5], lim = ag.dyn_params[6];
-      const float steer = fminf(fmaxf(u[1], -lim), lim), v = u[0];
-      d = integrate_pose(yaw, dt, rk4, [&](float h) { return bicycle_f(h, steer, v, l_f, l_r); });
+      d = bicycle_pose(u[0], u[1], yaw, dt, rk4, ag.dyn_params[4], ag.dyn_params[5], ag.dyn_params[6]);
     } else {  // drone: thrust gets the hover feed-forward (in place on the action, as the reference does)
       const float Ixx = ag.dyn_params[4], Iyy = ag.dyn_params[5], Izz = ag.dyn_params[6], g = ag.dyn_params[7];
       u[0] = u[0] + mass * g;
@@ -229,12 +264,7 @@ DEVI void ingest_actions_body(const IngestArgs& a, const long idx) {
       d.y = delta.v[7];
       d.yaw = delta.v[5];
     }
-    // the force / torque that realise the pose change under the world's integrator (dynamics/common)
-    const float2 vel = reinterpret_cast<const float2*>(a.st.vel)[ent];
-    const float w0 = a.st.ang_vel[ent];
-    const float dt2 = dt * dt;
-    force = make_float2(mass * ((d.x - vel.x * dt) / dt2), mass * ((d.y - vel.y * dt) / dt2));
-    torque = inertia * ((d.yaw - w0 * dt) / dt2);
+    force = kinematic_force(d, dt, mass, inertia, reinterpret_cast<const float2*>(a.st.vel)[ent], a.st.ang_vel[ent], torque);
     write_force = write_torque = true;
   }
 #pragma unroll

@@ -53,21 +53,39 @@ struct EpiArgs {
   void* obs_out;  // [rows, B, width] of P::OBS_DTYPE (fp32, fp16 or bf16), or null
   void* buffers[VMAS_PROG_MAX_BUFFERS];
 };
-// ... and its prologue (see spec_ingest_lane): the policy agents' holonomic actions, continuous, discrete or
-// multi-discrete
+// ... and its prologue (see spec_ingest_lane, spec_act_lane): the policy agents' actions, continuous, discrete or
+// multi-discrete, through their action model (holonomic, with rotation, forward, rotation, differential drive)
 struct ActC {
   int agent;  // row of the agent in the force / torque slab
   float range0, range1, mult0, mult1;
   int kind = VMAS_ACT_CONTINUOUS;  // VMAS_ACT_*
   int n0 = 0, n1 = 0;              // (discrete kinds) choices per component
+  int dyn = VMAS_DYN_HOLONOMIC;    // VMAS_DYN_*
+  int size = 2;                    // action components: the model's own, 1-4
+  float range2 = 0.f, range3 = 0.f, mult2 = 0.f, mult3 = 0.f;
+  int n2 = 0, n3 = 0;
+  float params[8] = {};  // the model's parameters (VmasAgentActions::dyn_params)
 };
+// a holonomic agent with 2 components: its rounds run the lean decode of spec_ingest_lane
+__host__ __device__ constexpr bool act_holonomic2(const ActC& c) { return c.dyn == VMAS_DYN_HOLONOMIC && c.size == 2; }
+__host__ __device__ constexpr float act_range(const ActC& c, int j) {
+  return j == 0 ? c.range0 : j == 1 ? c.range1 : j == 2 ? c.range2 : c.range3;
+}
+__host__ __device__ constexpr float act_mult(const ActC& c, int j) {
+  return j == 0 ? c.mult0 : j == 1 ? c.mult1 : j == 2 ? c.mult2 : c.mult3;
+}
+__host__ __device__ constexpr int act_n(const ActC& c, int j) { return j == 0 ? c.n0 : j == 1 ? c.n1 : j == 2 ? c.n2 : c.n3; }
 struct ActArgs {
-  const float* actions[VMAS_MAX_INGEST_AGENTS];  // the caller's tensors: fp32 [B, 2], or int64 [B, 1] / [B, 2]
-  float* u[VMAS_MAX_INGEST_AGENTS];              // [B, 2] each: agent.action.u
+  const float* actions[VMAS_MAX_INGEST_AGENTS];  // the caller's tensors: fp32 [B, size], or int64 [B, 1] / [B, size]
+  float* u[VMAS_MAX_INGEST_AGENTS];              // [B, size] each: agent.action.u
   uint8_t* bad_flag;
   float* steps;  // [B] or null
   int clamp;
-  int kind[VMAS_MAX_INGEST_AGENTS];  // VMAS_ACT_* of each agent's tensor: launch_env refuses one it was not built for
+  // what each agent's tensors are (launch_env refuses a combination it was not built for): VMAS_ACT_*, VMAS_DYN_*,
+  // the action size.  One byte each: the kernel never reads them, and every byte here is a byte of every launch.
+  int8_t kind[VMAS_MAX_INGEST_AGENTS];
+  int8_t dyn[VMAS_MAX_INGEST_AGENTS];
+  int8_t size[VMAS_MAX_INGEST_AGENTS];
 };
 struct alignas(16) ActIdx2 {  // one multi-discrete env row, loaded as one 16-byte word
   long long i0, i1;
@@ -737,16 +755,18 @@ DEVI void spec_integrate(EnvRegs<E>& r, const int sub, const SpecEnvParams<W>* p
 
 // The rows of one env (pos, vel, rot, ang_vel, agent force, agent torque) and which vector chunks
 // of them are read / written: derived from the world's entity flags at compile time.
-// ALL_FORCE: every movable agent's force columns are stored (the whole-step kernel ingests the actions itself)
-template <class W, bool ALL_FORCE = false>
+// ALL_FORCE: every movable agent's force columns are stored (the whole-step kernel ingests the actions itself);
+// F_ACT / T_ACT: the force / torque columns its action prologue writes, stored too (see spec_act_cols)
+template <class W, bool ALL_FORCE = false, uint64_t F_ACT = 0, uint64_t T_ACT = 0>
 struct SpecRows {
   static constexpr int E = W::E, NA = W::A;
   static constexpr uint64_t ALL_POS = (2 * E >= 64) ? ~0ull : ((1ull << (2 * E)) - 1);
   static constexpr uint64_t MOV2 = ent_cols<W>(VMAS_F_MOVABLE, 2);
   static constexpr uint64_t ROT1 = ent_cols<W>(VMAS_F_ROTATABLE, 1);
   static constexpr uint64_t F_DIRTY =
-      ALL_FORCE ? agent_cols<W>(VMAS_F_MOVABLE, 0, 2) : agent_cols<W>(VMAS_F_MOVABLE, VMAS_F_MAX_F | VMAS_F_F_RANGE, 2);
-  static constexpr uint64_t T_DIRTY = agent_cols<W>(VMAS_F_ROTATABLE, VMAS_F_MAX_T | VMAS_F_T_RANGE, 1);
+      (ALL_FORCE ? agent_cols<W>(VMAS_F_MOVABLE, 0, 2) : agent_cols<W>(VMAS_F_MOVABLE, VMAS_F_MAX_F | VMAS_F_F_RANGE, 2)) |
+      F_ACT;
+  static constexpr uint64_t T_DIRTY = agent_cols<W>(VMAS_F_ROTATABLE, VMAS_F_MAX_T | VMAS_F_T_RANGE, 1) | T_ACT;
   // a vector chunk that will be stored must have been loaded whole (it carries unchanged columns)
   static constexpr uint64_t VEL_IO = chunk_closure(MOV2, 2 * E, RowVec<2 * E>::W);
   static constexpr uint64_t ROT_ST = chunk_closure(ROT1, E, RowVec<E>::W);
@@ -819,11 +839,13 @@ struct SpecRows {
         w[e] = r.w[e];
       }
       if constexpr (en.flags & VMAS_F_AGENT) {
-        if constexpr ((en.flags & VMAS_F_MOVABLE) && (ALL_FORCE || (en.flags & (VMAS_F_MAX_F | VMAS_F_F_RANGE)))) {
+        if constexpr (((en.flags & VMAS_F_MOVABLE) && (ALL_FORCE || (en.flags & (VMAS_F_MAX_F | VMAS_F_F_RANGE)))) ||
+                      ((F_ACT >> (2 * en.agent)) & 3ull)) {
           f[2 * en.agent] = afx[en.agent];
           f[2 * en.agent + 1] = afy[en.agent];
         }
-        if constexpr ((en.flags & VMAS_F_ROTATABLE) && (en.flags & (VMAS_F_MAX_T | VMAS_F_T_RANGE)))
+        if constexpr (((en.flags & VMAS_F_ROTATABLE) && (en.flags & (VMAS_F_MAX_T | VMAS_F_T_RANGE))) ||
+                      ((T_ACT >> en.agent) & 1ull))
           t[en.agent] = atq[en.agent];
       }
     });
@@ -1132,6 +1154,128 @@ DEVI void spec_ingest_put(const float2 u, const float2 p, const bool odd, float*
   }
 }
 
+// ---- the prologue's rounds with other action models (any round with an agent that is not holonomic with 2
+// components).  Each lane runs its own agent's decode and model under a branch on the lane: the agents of a pair may
+// differ in model and action kind.  A lane hands its partner the force and the torque it computed.
+struct ActBody {  // the state an action model reads: the agent's heading, angular velocity and velocity
+  float rot, w;
+  float2 vel;
+};
+struct ActOut {  // what it returns: the force and torque rows
+  float2 f;
+  float t;
+};
+
+// the force / torque columns (width 2 / 1) that the prologue of P writes
+template <class P>
+__host__ __device__ constexpr uint64_t spec_act_cols(bool torque) {
+  uint64_t m = 0;
+  for (int k = 0; k < P::N_ACT; ++k) {
+    const ActC& c = P::act[k];
+    if (torque ? dyn_writes_torque(c.dyn) : dyn_writes_force(c.dyn)) m |= (torque ? 1ull : 3ull) << ((torque ? 1 : 2) * c.agent);
+  }
+  return m;
+}
+// round J runs spec_ingest_lane (both agents holonomic with 2 components and of one kind), else spec_act_lane
+template <class P, int G, int J>
+__host__ __device__ constexpr bool spec_act_lean() {
+  constexpr ActC c0 = P::act[SpecActRound<P, G, J>::k0], c1 = P::act[SpecActRound<P, G, J>::k1];
+  return act_holonomic2(c0) && act_holonomic2(c1) && c0.kind == c1.kind;
+}
+
+// Agent k's action: decoded as ingest_actions_body decodes it (the same helpers, the same unravel order), through
+// its model (act_model, the ingest kernel's device functions).  u is stored to agent.action.u if `store_u`.
+// `body(std::integral_constant<int, k>{})`: the agent's ActBody (read only by the models that need it).
+template <class P, int k, class Body>
+DEVI ActOut spec_act_agent(const ActArgs& act, const long env, const bool store_u, bool& bad, Body&& body) {
+  constexpr ActC c = P::act[k];
+  constexpr int sz = c.size;
+  float u[VMAS_MAX_ACTION_SIZE];
+  if constexpr (c.kind == VMAS_ACT_CONTINUOUS) {
+    const float* in = act.actions[k] + (size_t)env * sz;
+    static_for<sz>([&](auto ji) {
+      constexpr int j = decltype(ji)::value;
+      u[j] = ingest_continuous(in[j], act_range(c, j), act_mult(c, j), act.clamp, bad);
+    });
+  } else {
+    const long long* idx_in = reinterpret_cast<const long long*>(act.actions[k]);
+    long long flat = c.kind == VMAS_ACT_DISCRETE ? idx_in[env] : 0;
+    static_for<sz>([&](auto ji) {
+      constexpr int j = decltype(ji)::value;
+      constexpr ActC c = P::act[k];  // (the enclosing one is not a constant in here)
+      long long i;
+      if constexpr (c.kind == VMAS_ACT_DISCRETE) {  // unravel the flat index of the cartesian product
+        long long stride = 1;
+        for (int m = j + 1; m < sz; ++m) stride *= act_n(c, m);
+        i = flat / stride;
+        flat = flat % stride;
+      } else {
+        i = idx_in[(size_t)env * sz + j];
+      }
+      u[j] = ingest_discrete(i, act_n(c, j), act_range(c, j), act_mult(c, j), bad);
+    });
+  }
+  ActOut o;
+  o.f = make_float2(0.f, 0.f);
+  o.t = 0.f;
+  if constexpr (c.dyn == VMAS_DYN_HOLONOMIC || c.dyn == VMAS_DYN_HOLONOMIC_ROT) {
+    o.f = make_float2(u[0], u[1]);
+    if constexpr (c.dyn == VMAS_DYN_HOLONOMIC_ROT) o.t = u[2];
+  } else if constexpr (c.dyn == VMAS_DYN_FORWARD) {
+    o.f = forward_force(u[0], body(std::integral_constant<int, k>{}).rot);
+  } else if constexpr (c.dyn == VMAS_DYN_ROTATION) {
+    o.t = u[0];
+  } else {
+    static_assert(c.dyn == VMAS_DYN_DIFF_DRIVE, "an action model the prologue has not (codegen.PROLOGUE_MODELS)");
+    const ActBody b = body(std::integral_constant<int, k>{});
+    const float dt = c.params[0], mass = c.params[1], inertia = c.params[2];
+    constexpr bool rk4 = c.params[3] != 0.f;
+    const Pose3 d = diff_drive_pose(u[0], u[1], b.rot, dt, rk4);
+    o.f = kinematic_force(d, dt, mass, inertia, b.vel, b.w, o.t);
+  }
+  if (store_u) {
+    static_for<sz>([&](auto ji) {
+      constexpr int j = decltype(ji)::value;
+      act.u[k][(size_t)env * sz + j] = u[j];
+    });
+  }
+  return o;
+}
+
+// The lane's agent of round J (k1 on the odd lane of a pair, else k0; a lone agent: both lanes, the even one stores)
+template <class P, int G, int J, class Body>
+DEVI ActOut spec_act_lane(const ActArgs& act, const long env, const bool odd, const bool live, bool& bad, Body&& body) {
+  constexpr int k0 = SpecActRound<P, G, J>::k0, k1 = SpecActRound<P, G, J>::k1;
+  if constexpr (k0 == k1) {
+    return spec_act_agent<P, k0>(act, env, live && !odd, bad, body);
+  } else {
+    if (odd) return spec_act_agent<P, k1>(act, env, live, bad, body);
+    return spec_act_agent<P, k0>(act, env, live, bad, body);
+  }
+}
+
+// ... and round J's rows on the lane: own = its result, p = the partner lane's (a pair of agents only).  Only the
+// rows each model writes.
+template <class P, int G, int J>
+DEVI void spec_act_put(const ActOut& own, const ActOut& p, const bool odd, float* afx, float* afy, float* atq) {
+  constexpr int k0 = SpecActRound<P, G, J>::k0, k1 = SpecActRound<P, G, J>::k1;
+  constexpr ActC c0 = P::act[k0], c1 = P::act[k1];
+  const ActOut& r0 = k0 == k1 || !odd ? own : p;
+  if constexpr (dyn_writes_force(c0.dyn)) {
+    afx[c0.agent] = r0.f.x;
+    afy[c0.agent] = r0.f.y;
+  }
+  if constexpr (dyn_writes_torque(c0.dyn)) atq[c0.agent] = r0.t;
+  if constexpr (k0 != k1) {
+    const ActOut& r1 = odd ? own : p;
+    if constexpr (dyn_writes_force(c1.dyn)) {
+      afx[c1.agent] = r1.f.x;
+      afy[c1.agent] = r1.f.y;
+    }
+    if constexpr (dyn_writes_torque(c1.dyn)) atq[c1.agent] = r1.t;
+  }
+}
+
 #ifdef __CUDACC__
 // SCHED: the env-scheduling variant (thread t steps env order[t], signatures recorded); the default
 // kernel carries none of that code
@@ -1200,8 +1344,8 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_fused_kernel(con
 
 // ---- the whole Environment.step as ONE kernel -----------------------------------------------------------
 // step_fused_kernel plus what the ingest launch in front of it does (vmas_b200_ingest_actions_broad_phase):
-// every thread decodes its env's actions (holonomic; continuous, discrete or multi-discrete: ref
-// environment.py:616-707 and dynamics/holonomic.py:14-15) straight into the force registers, counts the step, and tests its env's
+// every thread decodes its env's actions (continuous, discrete or multi-discrete: ref environment.py:616-707; through
+// each agent's action model, ref dynamics/*.py) straight into the force / torque registers, counts the step, and tests its env's
 // masked pairs for the batch-wide broad phase (ref core.py:2797-2801); the mask is complete once every block
 // has contributed — a grid-wide barrier, which needs all blocks resident (cooperative launch; the launcher
 // says no for batches beyond that and the caller keeps the separate ingest launch).
@@ -1232,6 +1376,14 @@ __host__ __device__ constexpr int spec_n_masked() {
   int n = 0;
   for (int i = 0; i < W::NI; ++i) n += W::item[i].mask_bit >= 0;
   return n;
+}
+
+// the entity of agent row `agent`
+template <class W>
+__host__ __device__ constexpr int spec_agent_entity(int agent) {
+  for (int e = 0; e < W::E; ++e)
+    if ((W::ent[e].flags & VMAS_F_AGENT) && W::ent[e].agent == agent) return e;
+  return -1;
 }
 
 // the partner lane's value (lanes 2k, 2k + 1)
@@ -1271,7 +1423,7 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
   const bool odd = G > 1 && (threadIdx.x & 1);
   const bool live = tid < a.batch_dim;
   const long env = live ? tid : (long)a.batch_dim - 1;  // (the tail threads shadow the last env and store nothing)
-  SpecRows<W, true> rows;
+  SpecRows<W, true, spec_act_cols<P>(false), spec_act_cols<P>(true)> rows;
   rows.load_pos_rot(a, env);
   rows.load_rest(a, env);
   spec_epilogue_prefetch<P>(e, env);
@@ -1286,11 +1438,38 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
   bool bad = false;
   static_for<(P::N_ACT + G - 1) / G>([&](auto ji) {
     constexpr int J = decltype(ji)::value;
-    const float2 u = spec_ingest_lane<P, G, J>(act, env, odd, live, bad);
-    if constexpr (SpecActRound<P, G, J>::k0 == SpecActRound<P, G, J>::k1)
-      spec_ingest_put<P, G, J>(u, u, odd, afx, afy);
-    else
-      spec_ingest_put<P, G, J>(u, make_float2(pair_swap(u.x), pair_swap(u.y)), odd, afx, afy);
+    constexpr int k0 = SpecActRound<P, G, J>::k0, k1 = SpecActRound<P, G, J>::k1;
+    if constexpr (spec_act_lean<P, G, J>()) {
+      const float2 u = spec_ingest_lane<P, G, J>(act, env, odd, live, bad);
+      if constexpr (k0 == k1)
+        spec_ingest_put<P, G, J>(u, u, odd, afx, afy);
+      else
+        spec_ingest_put<P, G, J>(u, make_float2(pair_swap(u.x), pair_swap(u.y)), odd, afx, afy);
+    } else {
+      // the models read the agent's state from the registers loaded above (nothing has moved yet); an entity whose
+      // heading or velocities the substeps do not use has them in the slab only
+      auto body = [&](auto ki) {
+        constexpr int ent = spec_agent_entity<W>(P::act[decltype(ki)::value].agent);
+        constexpr int f = W::ent[ent].flags;
+        const size_t at = (size_t)env * E + ent;
+        ActBody b;
+        if constexpr (f & (VMAS_F_TRIG | VMAS_F_ROTATABLE)) b.rot = r.rot[ent];
+        else b.rot = a.st.rot[at];
+        if constexpr (f & VMAS_F_ROTATABLE) b.w = r.w[ent];
+        else b.w = a.st.ang_vel[at];
+        if constexpr (f & VMAS_F_MOVABLE) b.vel = make_float2(r.vx[ent], r.vy[ent]);
+        else b.vel = reinterpret_cast<const float2*>(a.st.vel)[at];
+        return b;
+      };
+      const ActOut own = spec_act_lane<P, G, J>(act, env, odd, live, bad, body);
+      ActOut p = own;
+      if constexpr (k0 != k1) {
+        constexpr ActC c0 = P::act[k0], c1 = P::act[k1];
+        if constexpr (dyn_writes_force(c0.dyn) || dyn_writes_force(c1.dyn)) p.f = make_float2(pair_swap(own.f.x), pair_swap(own.f.y));
+        if constexpr (dyn_writes_torque(c0.dyn) || dyn_writes_torque(c1.dyn)) p.t = pair_swap(own.t);
+      }
+      spec_act_put<P, G, J>(own, p, odd, afx, afy, atq);
+    }
   });
   if constexpr (G > 1) bad = __shfl_xor_sync(0xffffffffu, (int)bad, 1) || bad;
   if (live && !odd) {
@@ -1431,8 +1610,9 @@ static cudaError_t launch_env_lanes(const SpecArgs& a, const EpiArgs& e, const A
 // at once even so (masked worlds only)
 template <class W, class P>
 static cudaError_t launch_env(const SpecArgs& a, const EpiArgs& e, const ActArgs& act, cudaStream_t stream) {
-  for (int k = 0; k < P::N_ACT; ++k)  // (the kernel reads each agent's tensor as the kind it was compiled for)
-    if (act.kind[k] != P::act[k].kind) return cudaErrorInvalidValue;
+  for (int k = 0; k < P::N_ACT; ++k)  // (the kernel reads each agent's tensors as what it was compiled for)
+    if (act.kind[k] != P::act[k].kind || act.dyn[k] != P::act[k].dyn || act.size[k] != P::act[k].size)
+      return cudaErrorInvalidValue;
   const long blocks = ((long)a.batch_dim + W::BLOCK - 1) / W::BLOCK;
   const bool coop = W::MASK_WORDS > 0 && a.use_mask;
   long cap = 0;

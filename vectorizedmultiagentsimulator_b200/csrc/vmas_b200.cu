@@ -2171,20 +2171,25 @@ static int env_step_one_kernel(const VmasEnvStep* s, const StepTargets& t, cudaS
   args.n_substeps = s->cfg->substeps;
   ActArgs act;
   if (s->n_agents > VMAS_MAX_INGEST_AGENTS) return 0;
-  for (int i = 0; i < VMAS_MAX_INGEST_AGENTS; ++i) act.kind[i] = -1;  // (no tensor)
+  for (int i = 0; i < VMAS_MAX_INGEST_AGENTS; ++i) act.kind[i] = act.dyn[i] = act.size[i] = -1;  // (no tensor)
   for (int i = 0; i < s->n_agents; ++i) {
     const VmasAgentActions& ag = s->agents[i];
     if (!ag.actions || !ag.u) return fail("null action buffer%s");
-    if (ag.dynamics != VMAS_DYN_HOLONOMIC || ag.action_size != 2) return 0;
-    // fp32 [B, 2] and int64 [B, 1] rows are read as 8-byte words, int64 [B, 2] rows as 16-byte words
-    const uintptr_t align = ag.action_kind == VMAS_ACT_MULTIDISCRETE ? 15u : 7u;
+    if (ag.action_size < 1 || ag.action_size > 4) return 0;
+    // holonomic agents with 2 components: fp32 [B, 2] and int64 [B, 1] rows are read as 8-byte words, int64
+    // [B, 2] rows as 16-byte words; other models read their [B, 1..4] rows one element at a time
+    const bool lean = ag.dynamics == VMAS_DYN_HOLONOMIC && ag.action_size == 2;
+    const uintptr_t align = !lean ? (ag.action_kind == VMAS_ACT_CONTINUOUS ? 3u : 7u)
+                                  : ag.action_kind == VMAS_ACT_MULTIDISCRETE ? 15u : 7u;
     if (ag.action_kind != VMAS_ACT_CONTINUOUS && ag.action_kind != VMAS_ACT_DISCRETE &&
         ag.action_kind != VMAS_ACT_MULTIDISCRETE)
       return 0;
-    if (((uintptr_t)ag.actions & align) || ((uintptr_t)ag.u & 7u)) return 0;
+    if (((uintptr_t)ag.actions & align) || ((uintptr_t)ag.u & (lean ? 7u : 3u))) return 0;
     act.actions[i] = ag.actions;
     act.u[i] = ag.u;
     act.kind[i] = ag.action_kind;
+    act.dyn[i] = ag.dynamics;
+    act.size[i] = ag.action_size;
   }
   act.bad_flag = s->bad_flag;
   act.steps = s->steps;

@@ -229,8 +229,7 @@ def request_step_kernel(desc: P.WorldDescription, cols, instrs, acts=(), block: 
                         obs_dtype: int = 0) -> Optional[StepKernelJob]:
     """Starts (or finds) the compilation of the whole-step kernel; None if the world cannot be specialised or
     has per-env physical parameters (those step on the captured graph of the specialised substep kernel).
-    ``acts``: [(agent row, u_range x 2, u_multiplier x 2)] of the policy agents if the kernel is to ingest
-    their (holonomic) actions itself; discrete and multi-discrete agents append (``VMAS_ACT_*`` kind, nvec x 2).
+    ``acts``: ``codegen.prologue_acts`` of the policy agents if the kernel is to ingest their actions itself.
     ``prebuild_step_kernels`` compiles the continuous variants only.  ``obs_dtype``: the type the kernel stores its observation
     rows as (``VMAS_DTYPE_*``; part of the key)."""
     if not available() or not codegen.specializable(desc):
@@ -285,15 +284,19 @@ def prebuild_step_kernels(verbose: bool = False):
         # environment adds one STORE per result leaf to the program when it captures its step, so its own
         # variant is compiled then (seconds) — these two make sure the templates build, and serve
         # VMAS_B200_RESULTS_IN_PLACE=0
-        from .simulator.dynamics.basic import Holonomic
+        from types import SimpleNamespace
 
-        agents = world.policy_agents
-        holonomic = all(type(a.dynamics) is Holonomic and a.action_size == 2 for a in agents)
         row = {id(a): j for j, a in enumerate(world.agents)}
-        acts = tuple(
-            (row[id(a)], *(float(v) for v in a.action.u_range_tensor.tolist()), *(float(v) for v in a.action.u_multiplier_tensor.tolist()))
-            for a in agents
-        ) if holonomic else ()
+        agents = []
+        for a in world.policy_agents:
+            dyn = codegen.dynamics_code(a.dynamics)
+            if a.action_size == 0 and dyn == _native.DYN_NONE:
+                continue  # (static agents: nothing to ingest)
+            agents.append(SimpleNamespace(
+                agent_index=row[id(a)], dynamics=-2 if dyn is None else dyn, action_size=a.action_size,
+                u_range=a.action.u_range_tensor.tolist(), u_multiplier=a.action.u_multiplier_tensor.tolist(), nvec=(),
+                dyn_params=codegen.dynamics_params(a, -2 if dyn is None else dyn)))
+        acts = codegen.prologue_acts(agents)
         for variant in ((), acts) if acts else ((),):
             job = StepKernelJob(desc, columns, instrs, variant, out_dir=PREBUILT_DIR)
             job.run()

@@ -497,16 +497,7 @@ class Environment(TorchVectorizedObject):
         if cached is not None and cached[0] == version:
             return cached[1]
         from ... import _native as N
-        from ..dynamics.basic import Forward, Holonomic, HolonomicWithRotation, Rotation, Static
-        from ..dynamics.diff_drive import DiffDrive
-        from ..dynamics.drone import Drone
-        from ..dynamics.kinematic_bicycle import KinematicBicycle
-
-        codes = {
-            Holonomic: N.DYN_HOLONOMIC, HolonomicWithRotation: N.DYN_HOLONOMIC_ROT, Forward: N.DYN_FORWARD,
-            Rotation: N.DYN_ROTATION, Static: N.DYN_NONE, DiffDrive: N.DYN_DIFF_DRIVE,
-            KinematicBicycle: N.DYN_BICYCLE, Drone: N.DYN_DRONE,
-        }
+        from ... import codegen
 
         specs = None
         ok = (
@@ -520,7 +511,7 @@ class Environment(TorchVectorizedObject):
             for agent in self.agents:
                 noise = agent.action.u_noise
                 noisy = (max(noise) if isinstance(noise, Sequence) else noise) > 0
-                dyn = codes.get(type(agent.dynamics))  # exact types: a subclass may override process_action
+                dyn = codegen.dynamics_code(agent.dynamics)  # exact types: a subclass may override process_action
                 size_ok = 0 < agent.action_size <= 8 or (agent.action_size == 0 and dyn == N.DYN_NONE)
                 if noisy or dyn is None or self._comm_dims(agent) > 0 or not size_ok:
                     specs = None
@@ -946,29 +937,23 @@ class Environment(TorchVectorizedObject):
             if _WHOLE_STEP_KERNEL and backend._dev_tables.tb.specialization >= 0:
                 # the whole-step kernel of this (world, program, observation plan): compiled once (seconds),
                 # cached on disk; until it is there the step runs as two launches — same bits
-                from ... import jit
+                from ... import codegen, jit
 
                 cols_np = None if cols is None else oplan.compile(self.world)[0]
                 if cols_np is not None:
-                    from ... import codegen
-
                     cols_np = codegen.fuse_value_columns(cols_np, oplan.buffer_sources, instrs)
-                # ... with the action ingest (and the broad phase) as its prologue where the agents allow it:
-                # the whole step is then ONE launch.  Continuous, discrete and multi-discrete spaces alike.
+                # ... with the action ingest (and the broad phase) as its prologue where the agents allow it
+                # (codegen.prologue_acts: their action models; static agents have nothing to ingest): the whole
+                # step is then ONE launch.  Continuous, discrete and multi-discrete spaces alike.
                 acts = ()
                 if (
-                    _INGEST_IN_KERNEL and len(live) == len(specs)
-                    and all(s[1] == N.DYN_HOLONOMIC and s[0].action_size == 2 for s in specs)
+                    _INGEST_IN_KERNEL
                     and type(self.scenario).pre_step is BaseScenario.pre_step and not self.world.scripted_agents
                     and (ingest_built_mask or backend.tables.n_masked == 0 or not self.world.exact_broad_phase)
                 ):
-                    acts = tuple(
-                        (int(c.agent_index), float(c.u_range[0]), float(c.u_range[1]), float(c.u_multiplier[0]),
-                         float(c.u_multiplier[1]))
-                        + (() if self.continuous_actions else (int(c.action_kind), int(c.nvec[0]), int(c.nvec[1])))
-                        for c in arr
-                    )
-                    plan.c.ingest_in_kernel = 1
+                    acts = codegen.prologue_acts(arr, N.ACT_CONTINUOUS if self.continuous_actions else int(arr[0].action_kind))
+                    if acts:
+                        plan.c.ingest_in_kernel = 1
                 job = jit.request_step_kernel(backend.tables.desc, cols_np, instrs, acts, obs_dtype=obs_dtype)
                 if job is not None:
                     job.done.wait(timeout=_WHOLE_STEP_KERNEL_WAIT_S)
