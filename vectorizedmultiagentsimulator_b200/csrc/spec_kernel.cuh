@@ -1349,8 +1349,9 @@ __global__ void __launch_bounds__(W::BLOCK, W::MIN_BLOCKS) step_fused_kernel(con
 // masked pairs for the batch-wide broad phase (ref core.py:2797-2801); the mask is complete once every block
 // has contributed — a grid-wide barrier, which needs all blocks resident (cooperative launch; the launcher
 // says no for batches beyond that and the caller keeps the separate ingest launch).
-//   a.mask: per substep [MASK_WORDS] bits, [MASK_WORDS] arrivals at the barrier, [MASK_WORDS + 1] blocks done
-//   with the mask (substeps x (MASK_WORDS + 2) words, zero between launches)
+//   a.mask: per substep [MASK_WORDS] bits, [MASK_WORDS] arrivals at the barrier, [MASK_WORDS + 1] unused but for
+//   substep 0's, which counts the blocks done with every mask (substeps x (MASK_WORDS + 2) words, zero between
+//   launches)
 template <class W>
 __host__ __device__ constexpr int spec_first_masked() {
   for (int i = 0; i < W::NI; ++i)
@@ -1358,10 +1359,33 @@ __host__ __device__ constexpr int spec_first_masked() {
   return W::NI;
 }
 
+// word w of the mask with every masked item's bit set: the most the batch-wide OR can hold
+template <class W>
+__host__ __device__ constexpr uint32_t spec_mask_full(int w) {
+  uint32_t m = 0u;
+  for (int i = 0; i < W::NI; ++i)
+    if (W::item[i].mask_bit >= 0 && (W::item[i].mask_bit >> 5) == w) m |= 1u << (W::item[i].mask_bit & 31);
+  return m;
+}
+
 DEVI unsigned ld_acquire_u32(const uint32_t* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
+}
+
+// fire-and-forget: nothing comes back to wait on
+DEVI void red_or_u32(uint32_t* p, uint32_t v) {
+  asm volatile("red.relaxed.gpu.global.or.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// the release orders this thread's earlier stores and reductions (the mask bits) before the add
+DEVI void red_release_add_u32(uint32_t* p, uint32_t v) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+DEVI unsigned atom_acq_rel_add_u32(uint32_t* p, uint32_t v) {
+  unsigned old;
+  asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
+  return old;
 }
 
 // the k-th masked work item, in item order
@@ -1477,12 +1501,15 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
     if (act.steps) act.steps[env] = act.steps[env] + 1.f;
   }
   // The batch-wide broad phase of every substep, inside the kernel.  ARRIVE: the block's pairs-in-range bits go
-  // to the global mask of the substep and the block checks in at its barrier; WAIT only where the first masked
-  // work item is due — the trigonometry, the per-entity forces and the unmasked items in front of it (sphere
-  // pairs) run while the other blocks arrive.  Substep s uses a.mask + s * (MW + 2): [MW] bits, arrivals, blocks
-  // done with the mask (the last of them clears the region for the next step).
+  // to the global mask of the substep and the block checks in at its barrier, both as reductions that return
+  // nothing, so no thread waits on them.  WAIT only where the first masked work item is due — the trigonometry,
+  // the per-entity forces and the unmasked items in front of it (sphere pairs) run while the other blocks
+  // arrive — and only if the block's own envs left a masked bit unset: the batch-wide mask is the OR of every
+  // block's bits, so a block that has them all already holds it.  Substep s uses a.mask + s * (MW + 2): [MW]
+  // bits, arrivals; after the epilogue, the last block to finish clears every substep's region for the next step.
   uint32_t mask_words[MW > 0 ? MW : 1];
-  [[maybe_unused]] __shared__ uint32_t s_mask[MW > 0 ? MW : 1];
+  [[maybe_unused]] __shared__ uint32_t s_mask[MW > 0 ? MW : 1];   // the block's own bits
+  [[maybe_unused]] __shared__ uint32_t s_gmask[MW > 0 ? MW : 1];  // the batch-wide mask, where the block waited
   static_assert(MW <= W::BLOCK, "more mask words than threads in a block");
   uint32_t sig = 0;
   for (int sub = 0; sub < W::cfg.substeps; ++sub) {
@@ -1518,12 +1545,11 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
         }
         __syncthreads();
         if (threadIdx.x == 0) {
-          for (int w = 0; w < MW; ++w) {  // (bits only ever get set: a stale read costs one redundant atomic)
+          for (int w = 0; w < MW; ++w) {
             const uint32_t b = s_mask[w];
-            if (b && (ld_acquire_u32(&gmask[w]) & b) != b) atomicOr(&gmask[w], b);
+            if (b) red_or_u32(&gmask[w], b);
           }
-          __threadfence();
-          atomicAdd(&gmask[MW], 1u);
+          red_release_add_u32(&gmask[MW], 1u);
         }
       }
     }
@@ -1541,18 +1567,25 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
       constexpr int K = decltype(ki)::value;
       if constexpr (MW > 0 && R::template I0<K> == spec_first_masked<W>()) {
         if (a.use_mask) {  // WAIT
-          if (threadIdx.x == 0) {
-            while (ld_acquire_u32(&gmask[MW]) < gridDim.x) __nanosleep(20);
-            for (int w = 0; w < MW; ++w) s_mask[w] = ld_acquire_u32(&gmask[w]);
-            __threadfence();
-            const unsigned done = atomicAdd(&gmask[MW + 1], 1u);
-            if (done == gridDim.x - 1) {  // every block has its copy: clear for the next step
-              for (int w = 0; w < MW + 2; ++w) gmask[w] = 0u;
-            }
-          }
-          __syncthreads();
+          // (s_mask holds the block's own bits since ARRIVE's __syncthreads and stays put: every thread takes the
+          // same branch)
+          bool full = true;
+          static_for<MW>([&](auto wi) {
+            constexpr uint32_t all = spec_mask_full<W>(decltype(wi)::value);
+            full = full && s_mask[decltype(wi)::value] == all;
+          });
+          if (full) {
 #pragma unroll
-          for (int w = 0; w < MW; ++w) mask_words[w] = s_mask[w];
+            for (int w = 0; w < MW; ++w) mask_words[w] = s_mask[w];
+          } else {
+            if (threadIdx.x == 0) {
+              while (ld_acquire_u32(&gmask[MW]) < gridDim.x) __nanosleep(20);
+              for (int w = 0; w < MW; ++w) s_gmask[w] = s_mask[w] | ld_acquire_u32(&gmask[w]);
+            }
+            __syncthreads();
+#pragma unroll
+            for (int w = 0; w < MW; ++w) mask_words[w] = s_gmask[w];
+          }
         }
       }
       if constexpr (R::template I0<K> == R::template I1<K>) {  // a lone item: both lanes evaluate it
@@ -1571,6 +1604,17 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
     const float v0 = __shfl_xor_sync(0x3u << (threadIdx.x & 30), v, 1);  // (both lanes of a pair are here)
     return odd ? v0 : v;
   });
+  if constexpr (MW > 0) {
+    // thread 0 (always live: it owns the block's first env) is the only thread that touches a.mask.  Once every
+    // block has counted itself here, every block has arrived at every barrier and read every mask it waited for,
+    // so the last one clears all the regions: the release / acquire of the count orders those reads and
+    // arrivals before the clearing stores.
+    if (a.use_mask && threadIdx.x == 0) {
+      if (atom_acq_rel_add_u32(&a.mask[MW + 1], 1u) == gridDim.x - 1) {
+        for (int w = 0; w < W::cfg.substeps * (MW + 2); ++w) a.mask[w] = 0u;
+      }
+    }
+  }
 }
 
 // resident blocks of step_env_kernel<W, P, G> on the current device (occupancy query, once per device)
