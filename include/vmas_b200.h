@@ -271,6 +271,9 @@ int vmas_b200_gather_observations_buffers(const VmasWorldConfig* cfg, const Vmas
  *   ADD SUB MUL MIN MAX OR AND LT LE   dst <- a op b       NEG NOT   dst <- op a
  *   WHERE            dst <- a != 0 ? b : register (arg & 0xFF)
  *   STORE_F32 / STORE_BOOL   buffers[b][env] <- a
+ *   STEP_COUNT       dst <- the env's step counter after this step's increment; `a`: the buffer slot of the counter
+ *                    (Environment.steps).  A load of buffers[a][env] everywhere but in step_env_kernel, which counts
+ *                    the step in its prologue and hands the sum over in a register.
  * `columns`, `n_rows`, `width`, `obs_out`: as vmas_b200_gather_observations (or NULL / 0: program only).
  */
 #define VMAS_PROG_MAX_INSTR 64
@@ -279,7 +282,7 @@ int vmas_b200_gather_observations_buffers(const VmasWorldConfig* cfg, const Vmas
 enum {
   VMAS_OP_OVERLAP = 1, VMAS_OP_DISTANCE, VMAS_OP_CENTER_DISTANCE, VMAS_OP_SHAPING, VMAS_OP_LOAD_F32, VMAS_OP_LOAD_BOOL,
   VMAS_OP_CONST, VMAS_OP_ADD, VMAS_OP_SUB, VMAS_OP_MUL, VMAS_OP_MIN, VMAS_OP_MAX, VMAS_OP_NEG, VMAS_OP_OR, VMAS_OP_AND,
-  VMAS_OP_NOT, VMAS_OP_LT, VMAS_OP_LE, VMAS_OP_WHERE, VMAS_OP_STORE_F32, VMAS_OP_STORE_BOOL
+  VMAS_OP_NOT, VMAS_OP_LT, VMAS_OP_LE, VMAS_OP_WHERE, VMAS_OP_STORE_F32, VMAS_OP_STORE_BOOL, VMAS_OP_STEP_COUNT
 };
 typedef struct VmasProgInstr {
   uint8_t op, dst, a, b;

@@ -124,6 +124,8 @@ class CudaBackend(PlanRuntime):
         self.kernel_events = None
         #: while a list: the library launches of a step being captured, in order (Environment._capture)
         self.trace = None
+        #: while a list: the step programs run since Environment._finish_step began (its step limit reads their outputs)
+        self.step_programs = None
 
     # -- tables ----------------------------------------------------------------------------
     def on_new_tables(self):
@@ -342,6 +344,8 @@ class CudaBackend(PlanRuntime):
             cached = (self._plan_version, c)
             prog.device_cache[id(self)] = cached
         c = cached[1]
+        if self.step_programs is not None:
+            self.step_programs.append(prog)
         B = self.world.batch_dim
         for slot, buf in enumerate(prog.buffers):
             t = prog.resolve(buf)

@@ -938,10 +938,24 @@ struct EpiOneLane {
   DEVI float operator()(float v) const { return v; }
 };
 
-// from_lane0(v): the value v of lane 0 of the env's lanes (the shaping carry, read by lane 0 only: it overwrites it)
-template <class W, class P, class X = EpiOneLane>
+// STEP_COUNT where the counter has been bumped by an earlier launch: a load of it
+struct EpiLoadCount {
+  DEVI float operator()(const float* steps) const { return *steps; }
+};
+
+// P's program reads the step counter (VMAS_OP_STEP_COUNT: a step limit, Environment._limit_program)
+template <class P>
+__host__ __device__ constexpr bool epi_counts() {
+  for (int i = 0; i < P::N_PROG; ++i)
+    if (P::prog[i].op == VMAS_OP_STEP_COUNT) return true;
+  return false;
+}
+
+// from_lane0(v): the value v of lane 0 of the env's lanes (the shaping carry, read by lane 0 only: it overwrites it);
+// count(&steps[env]): the env's step counter after this step's increment
+template <class W, class P, class X = EpiOneLane, class N = EpiLoadCount>
 DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs& e, const long env,
-                        const int lanes = 1, const int lane = 0, X from_lane0 = {}) {
+                        const int lanes = 1, const int lane = 0, X from_lane0 = {}, N count = {}) {
   // the step program (ref scenarios/balance.py:197-263 as a StepProgram; see vmas_b200_post_step)
   float pr[VMAS_PROG_REGS];
 #pragma unroll
@@ -968,6 +982,8 @@ DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs
       pr[in.dst] = static_cast<const float*>(e.buffers[in.a])[env];
     } else if constexpr (in.op == VMAS_OP_LOAD_BOOL) {
       pr[in.dst] = static_cast<const uint8_t*>(e.buffers[in.a])[env] ? 1.f : 0.f;
+    } else if constexpr (in.op == VMAS_OP_STEP_COUNT) {
+      pr[in.dst] = count(static_cast<const float*>(e.buffers[in.a]) + env);
     } else if constexpr (in.op == VMAS_OP_CONST) {
       pr[in.dst] = in.imm;
     } else if constexpr (in.op == VMAS_OP_ADD) {
@@ -1496,9 +1512,24 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
     }
   });
   if constexpr (G > 1) bad = __shfl_xor_sync(0xffffffffu, (int)bad, 1) || bad;
-  if (live && !odd) {
-    if (bad && act.bad_flag) *act.bad_flag = 1;
-    if (act.steps) act.steps[env] = act.steps[env] + 1.f;
+  // a program that reads the step counter gets the sum from here: a reload in the epilogue would race the even
+  // lane's store on the odd lane (launch_env refuses such a kernel without a counter)
+  [[maybe_unused]] float count = 0.f;
+  if constexpr (epi_counts<P>()) {
+    if (live && !odd) {
+      if (bad && act.bad_flag) *act.bad_flag = 1;
+      count = act.steps[env] + 1.f;
+      act.steps[env] = count;
+    }
+    if constexpr (G > 1) {
+      const float even = pair_swap(count);
+      if (odd) count = even;
+    }
+  } else {
+    if (live && !odd) {
+      if (bad && act.bad_flag) *act.bad_flag = 1;
+      if (act.steps) act.steps[env] = act.steps[env] + 1.f;
+    }
   }
   // The batch-wide broad phase of every substep, inside the kernel.  ARRIVE: the block's pairs-in-range bits go
   // to the global mask of the substep and the block checks in at its barrier, both as reductions that return
@@ -1599,11 +1630,15 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
   }
   if (!live) return;
   rows.store(a, env, r, afx, afy, atq, G, odd ? 1 : 0);
-  spec_epilogue<W, P>(r, a, e, env, G, odd ? 1 : 0, [odd](float v) {
+  const auto from_lane0 = [odd](float v) {
     if constexpr (G == 1) return v;
     const float v0 = __shfl_xor_sync(0x3u << (threadIdx.x & 30), v, 1);  // (both lanes of a pair are here)
     return odd ? v0 : v;
-  });
+  };
+  if constexpr (epi_counts<P>())
+    spec_epilogue<W, P>(r, a, e, env, G, odd ? 1 : 0, from_lane0, [count](const float*) { return count; });
+  else
+    spec_epilogue<W, P>(r, a, e, env, G, odd ? 1 : 0, from_lane0);
   if constexpr (MW > 0) {
     // thread 0 (always live: it owns the block's first env) is the only thread that touches a.mask.  Once every
     // block has counted itself here, every block has arrived at every barrier and read every mask it waited for,
@@ -1657,6 +1692,7 @@ static cudaError_t launch_env(const SpecArgs& a, const EpiArgs& e, const ActArgs
   for (int k = 0; k < P::N_ACT; ++k)  // (the kernel reads each agent's tensors as what it was compiled for)
     if (act.kind[k] != P::act[k].kind || act.dyn[k] != P::act[k].dyn || act.size[k] != P::act[k].size)
       return cudaErrorInvalidValue;
+  if (epi_counts<P>() && !act.steps) return cudaErrorInvalidValue;  // (the program's count comes from the prologue)
   const long blocks = ((long)a.batch_dim + W::BLOCK - 1) / W::BLOCK;
   const bool coop = W::MASK_WORDS > 0 && a.use_mask;
   long cap = 0;

@@ -1074,7 +1074,10 @@ DEVI void post_step_program_body(const ProgArgs& p, const int tile_envs) {
           r[in.dst + 1] = d;
           *prev = shaping;
         } break;
-        case VMAS_OP_LOAD_F32: r[in.dst] = static_cast<const float*>(p.prog.buffers[in.a])[env]; break;
+        case VMAS_OP_LOAD_F32:
+        case VMAS_OP_STEP_COUNT:  // (the ingest launch in front of this one has counted the step)
+          r[in.dst] = static_cast<const float*>(p.prog.buffers[in.a])[env];
+          break;
         case VMAS_OP_LOAD_BOOL: r[in.dst] = static_cast<const uint8_t*>(p.prog.buffers[in.a])[env] ? 1.f : 0.f; break;
         case VMAS_OP_CONST: r[in.dst] = in.imm; break;
         case VMAS_OP_ADD: r[in.dst] = r[in.a] + r[in.b]; break;

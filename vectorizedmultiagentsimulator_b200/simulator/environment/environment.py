@@ -73,6 +73,50 @@ def _rebuild_outputs(node, fresh):
     return payload
 
 
+def splice_program(instrs, n_regs, n_slots, extra, feed_slot=None, feed_reg=None, count_slot=None):
+    """One step program out of ``instrs`` (``[(op, dst, a, b, arg, imm)]`` over ``n_regs`` registers and ``n_slots``
+    buffer slots) and ``extra`` behind it: ``extra``'s registers and buffer slots are numbered on from the first
+    program's; its load of slot ``feed_slot`` (a result of the first program) is dropped and its readers read register
+    ``feed_reg`` instead; its load of slot ``count_slot`` (the step counter) becomes ``OP_STEP_COUNT``.  ``extra`` may
+    use loads, constants, the elementwise ops and stores.  Returns ``(instructions, registers, {extra's slot: slot})``."""
+    from .. import program as SP
+
+    regs, slots, fresh = {}, {}, []
+
+    def reg(r):
+        return regs[r]
+
+    def slot(j):
+        return slots.setdefault(j, n_slots + len(slots))
+
+    def new_reg(r):
+        regs[r] = n_regs + len(fresh)
+        fresh.append(r)
+        return regs[r]
+
+    out = list(instrs)
+    for op, dst, a, b, arg, imm in extra:
+        if op in (SP.OP_LOAD_F32, SP.OP_LOAD_BOOL):
+            if a == feed_slot:
+                regs[dst] = feed_reg
+                continue
+            kind = SP.OP_STEP_COUNT if a == count_slot and op == SP.OP_LOAD_F32 else op
+            out.append((kind, new_reg(dst), slot(a), 0, 0, 0.0))
+        elif op == SP.OP_CONST:
+            out.append((op, new_reg(dst), 0, 0, 0, imm))
+        elif op in (SP.OP_NEG, SP.OP_NOT):
+            out.append((op, new_reg(dst), reg(a), 0, 0, 0.0))
+        elif op == SP.OP_WHERE:
+            out.append((op, new_reg(dst), reg(a), reg(b), reg(arg), 0.0))
+        elif SP.OP_ADD <= op <= SP.OP_LE:
+            out.append((op, new_reg(dst), reg(a), reg(b), 0, 0.0))
+        elif op in (SP.OP_STORE_F32, SP.OP_STORE_BOOL):
+            out.append((op, 0, reg(a), slot(b), 0, 0.0))
+        else:
+            raise ValueError(f"op {op} cannot be spliced")
+    return out, n_regs + len(fresh), slots
+
+
 @contextlib.contextmanager
 def local_seed(vmas_random_state):
     """Runs the body on the environment's private (torch-CPU, numpy, python) RNG streams."""
@@ -604,9 +648,16 @@ class Environment(TorchVectorizedObject):
         else:
             self.steps += 1
         if not self.auto_reset:
-            return self._get_from_scenario(
-                get_observations=True, get_infos=True, get_rewards=True, get_dones=True, clone=clone_outputs
-            )
+            backend = self.world._get_backend() if self.device.type == "cuda" else None
+            if backend is not None:
+                backend.step_programs = []  # (the programs whose outputs _done's step limit may read)
+            try:
+                return self._get_from_scenario(
+                    get_observations=True, get_infos=True, get_rewards=True, get_dones=True, clone=clone_outputs
+                )
+            finally:
+                if backend is not None:
+                    backend.step_programs = None
         # auto-reset: rewards / infos / dones describe the step that just ran; every env it finished
         # is reset on the device (mask = dones, no host sync) and the observations are taken
         # afterwards, so a finished env hands out the first observation of its next episode.  The
@@ -863,15 +914,24 @@ class Environment(TorchVectorizedObject):
             self._one_call_state = "probe" if self._one_call is not None else "off"
 
     def _library_only_step(self, graph, trace):
-        """``(exact_broad_phase mode, program struct, StepProgram, plan, columns, obs block)`` if the captured
+        """``(exact_broad_phase mode, program struct, StepProgram, plan, columns, obs block, limit)`` if the captured
         step consists of nothing but this library's ``World.step`` followed by one step program / observation
         launch — the graph then holds no torch kernel, and ``vmas_b200_env_step`` can issue those launches
-        itself (direct mode), or one whole-step kernel.  None otherwise."""
-        if not _DIRECT_STEP or trace is None or [t[0] for t in trace] != ["step", "post"]:
+        itself (direct mode), or one whole-step kernel.  ``limit``: ``(StepProgram, struct)`` of the environment's
+        step limit if its launch follows (``_limit_program``), else None.  None otherwise."""
+        kinds = None if trace is None else [t[0] for t in trace]
+        if not _DIRECT_STEP or kinds not in (["step", "post"], ["step", "post", "post"]):
             return None
-        (_, n_step, mode), (_, n_post, prog, plan, c, out) = trace
+        (_, n_step, mode), (_, n_post, prog, plan, c, out) = trace[:2]
+        limit, n_limit = None, 0
+        if len(trace) == 3:
+            _, n_limit, lprog, lplan, lc, _ = trace[2]
+            own = getattr(self, "_limit_prog", None)
+            if own is None or lprog is not own[1] or lplan is not None:
+                return None  # (a second program of the scenario's)
+            limit = (lprog, lc)
         values = plan is not None and bool(plan.buffer_sources)  # columns fed by the program: program, then gather
-        if n_post != (2 if values and prog is not None else 1) or n_step + n_post != self._graph_launches:
+        if n_post != (2 if values and prog is not None else 1) or n_step + n_post + n_limit != self._graph_launches:
             return None  # (LIDAR columns ride in a launch of their own; anything else the backend launched)
         if values and any(not hasattr(src, "_slot") or src not in prog.outputs for src in plan.buffer_sources):
             return None  # (value columns that are not outputs of this program)
@@ -886,7 +946,48 @@ class Environment(TorchVectorizedObject):
         if plan is not None:
             dev = plan.device_cache.get(id(backend))
             cols = dev["cols"] if dev is not None and dev["any_state"] else None
-        return mode, c, prog, plan, cols, out
+        return mode, c, prog, plan, cols, out, limit
+
+    def _splice_limit(self, c, prog, instrs, limit):
+        """The scenario's program (struct ``c``, ``prog``, its resolved instructions ``instrs``) with the step limit
+        ``limit = (StepProgram, struct)`` behind it as ONE program (``splice_program``): ``(struct, instructions,
+        merged)``, ``merged.outputs`` the outputs of both with their slots in the merged program.  None if the result
+        exceeds the program's registers, instructions or buffers, or ``terminated`` is not stored by ``prog``."""
+        import types
+
+        from ... import _native as N
+        from .. import program as SP
+
+        lprog, lc = limit
+        feed_reg = None
+        if lprog.feed_slot is not None:
+            store_of = {b: a for op, _, a, b, _, _ in instrs if op in (SP.OP_STORE_F32, SP.OP_STORE_BOOL)}
+            feed = lprog.resolve(lprog.buffers[lprog.feed_slot])
+            o = next((o for o in prog.outputs if o.tensor is feed and o._slot in store_of), None)
+            if o is None:
+                return None
+            feed_reg = store_of[o._slot]
+        merged, n_regs, slots = splice_program(
+            instrs, prog.n_regs, len(prog.buffers), lprog.instructions(None), lprog.feed_slot, feed_reg, lprog.count_slot
+        )
+        n_slots = len(prog.buffers) + len(slots)
+        if n_regs > SP.MAX_REGS or len(merged) > N.PROG_MAX_INSTR or n_slots > N.PROG_MAX_BUFFERS:
+            return None
+        c2 = N.StepProgramC()
+        ctypes.memmove(ctypes.addressof(c2), ctypes.addressof(c), ctypes.sizeof(c2))
+        for k, (op, dst, a, b, arg, imm) in enumerate(merged):
+            ins = c2.instr[k]
+            ins.op, ins.dst, ins.a, ins.b, ins.arg, ins.imm = op, dst, a, b, arg, imm
+        c2.n_instr = len(merged)
+        outputs = list(prog.outputs)
+        for old, new in slots.items():
+            c2.buffers[new] = lc.buffers[old]
+        for o in lprog.outputs:
+            moved = SP.Output(o.dtype)
+            moved.tensor, moved._slot = o.tensor, slots[o._slot]
+            outputs.append(moved)
+        return c2, merged, types.SimpleNamespace(outputs=outputs, buffers=[None] * n_slots)
+
     def _build_one_call_step(self, graph, ingest_built_mask: bool, trace=None):
         """Everything ``vmas_b200_env_step`` needs, marshalled once (None: this step does not fit the call)."""
         backend = self.world._get_backend()
@@ -904,6 +1005,13 @@ class Environment(TorchVectorizedObject):
         copy = self._graph_out_copy[0] if self._graph_out_copy else None
         items = [] if copy is None else [(src, block, offset) for src, (block, offset) in zip(copy.keep, copy.where)]
         direct = self._library_only_step(graph, trace)
+        spliced = None
+        if direct is not None and direct[6] is not None:
+            # the step limit joins the scenario's program; the whole-step kernel takes its count from the prologue
+            if counts:
+                spliced = self._splice_limit(direct[1], direct[2], direct[2].instructions(backend.index_of), direct[6])
+            if spliced is None:
+                direct = None  # (too large a program, or no counter: the step stays on the graph)
         job = None
         if direct is None:
             plan = N.EnvStepPlan(
@@ -913,15 +1021,18 @@ class Environment(TorchVectorizedObject):
                 block_kinds=self._graph_out_block_kinds,
             )
         else:
-            mode, c, prog, oplan, cols, out = direct
+            mode, c, prog, oplan, cols, out, limit = direct
             instrs = prog.instructions(backend.index_of)
+            merged = prog
+            if spliced is not None:
+                c, instrs, merged = spliced
             obs_to, mirrors = None, []
             if _WRITE_RESULTS_IN_PLACE:
                 # results the post stage can write straight into the step's fresh blocks instead of into static
                 # buffers that are then copied: the observation rows (if one leaf run covers the whole block),
                 # and every leaf that is an output of the program (one more STORE per leaf)
                 c, instrs, items, obs_to, mirrors = self._results_in_place(
-                    c, prog, instrs, items, cols, out, self._graph_out_block_kinds
+                    c, merged, instrs, items, cols, out, self._graph_out_block_kinds
                 )
             # the post stage rounds the observation rows itself where it writes them into the fresh block
             obs_dtype = N.DTYPE_F32 if obs_to is None else self._graph_out_block_kinds[obs_to[0]]
@@ -933,7 +1044,7 @@ class Environment(TorchVectorizedObject):
                 exact_broad_phase=mode, obs_to=obs_to, mirrors=mirrors, block_kinds=self._graph_out_block_kinds,
                 obs_dtype=obs_dtype,
             )
-            plan.keep += (prog, oplan)
+            plan.keep += (prog, oplan, limit)
             if _WHOLE_STEP_KERNEL and backend._dev_tables.tb.specialization >= 0:
                 # the whole-step kernel of this (world, program, observation plan): compiled once (seconds),
                 # cached on disk; until it is there the step runs as two launches — same bits
@@ -1073,6 +1184,15 @@ class Environment(TorchVectorizedObject):
 
     def _done(self, clone=True):
         terminated = self.scenario.done()
+        limit = self._limit_applies(terminated)
+        if limit is not None:
+            # the step limit as a step program: one library launch (and, captured, part of the whole-step kernel)
+            self._limit_input = terminated
+            limit.run()
+            out = limit.out.tensor
+            if clone:
+                terminated, out = terminated.clone(), out.clone()
+            return (terminated, out) if self.terminated_truncated else out
         if clone:
             terminated = terminated.clone()
         truncated = self.steps >= self.max_steps if self.max_steps is not None else None
@@ -1083,6 +1203,46 @@ class Environment(TorchVectorizedObject):
         if truncated is None:
             return terminated
         return terminated + truncated
+
+    def _limit_program(self):
+        """``max_steps`` and the terminated / truncated split as a step program of the environment's own: the same
+        statements as ``_done``'s torch ops, bit for bit (``steps >= max_steps`` compares in fp32, as torch does with
+        an fp32 counter).  ``.out`` is ``dones`` (``terminated_truncated=False``) or ``truncated``.  Built again when
+        the limit changes; a captured step keeps the one it was captured with."""
+        from .. import program as SP
+
+        key = (self.max_steps, self.terminated_truncated)
+        cached = getattr(self, "_limit_prog", None)
+        if cached is not None and cached[0] == key and cached[1].world is self.world:
+            return cached[1]
+        p = SP.StepProgram(self.world)
+        p.count_slot = p.feed_slot = None  # buffer slots of the counter and of terminated (_splice_limit)
+        if self.max_steps is None:
+            p.out = p.store(p.const(0.0), torch.bool)
+        else:
+            count = p.load(lambda: self.steps)
+            p.count_slot = len(p.buffers) - 1
+            truncated = p.le(p.const(float(self.max_steps)), count)
+            if not self.terminated_truncated:
+                terminated = p.load(lambda: self._limit_input, is_bool=True)
+                p.feed_slot = len(p.buffers) - 1
+                truncated = p.logical_or(terminated, truncated)
+            p.out = p.store(truncated, torch.bool)
+        p.finalize()
+        self._limit_prog = (key, p)
+        return p
+
+    def _limit_applies(self, terminated):
+        """The limit program if ``_done`` runs it in place of its torch ops: on CUDA, inside a step (no auto-reset),
+        for a limit or a split, when ``terminated`` is an output of a step program of this step.  None otherwise."""
+        if self.max_steps is None and not self.terminated_truncated:
+            return None
+        programs = getattr(self.world._get_backend(), "step_programs", None)
+        if not programs or self.steps.dtype != torch.float32 or not self.steps.is_contiguous():
+            return None
+        if not any(o.tensor is terminated and o.dtype == torch.bool for prog in programs for o in prog.outputs):
+            return None
+        return self._limit_program()
 
     # ------------------------------------------------------------------------------------
     # spaces

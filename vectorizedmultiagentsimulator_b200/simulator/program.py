@@ -32,6 +32,10 @@ from torch import Tensor
     OP_OVERLAP, OP_DISTANCE, OP_CENTER_DISTANCE, OP_SHAPING, OP_LOAD_F32, OP_LOAD_BOOL, OP_CONST, OP_ADD, OP_SUB, OP_MUL,
     OP_MIN, OP_MAX, OP_NEG, OP_OR, OP_AND, OP_NOT, OP_LT, OP_LE, OP_WHERE, OP_STORE_F32, OP_STORE_BOOL,
 ) = range(1, 22)
+#: the env's step counter after this step's increment (operand ``a``: the counter's buffer slot).  A load of that
+#: buffer but in the one-kernel step, which counts the step itself; only ``Environment`` splices it into a program
+#: that step kernel runs (``_splice_limit``)
+OP_STEP_COUNT = 22
 MAX_INSTR, MAX_BUFFERS, MAX_REGS = 64, 16, 32
 
 Buffer = Union[Tensor, Callable[[], Tensor]]
