@@ -44,6 +44,7 @@ HEADERS = [
     os.path.join(CSRC, "generic_step.cuh"),
     os.path.join(CSRC, "query.cuh"),
     os.path.join(CSRC, "ingest.cuh"),
+    os.path.join(CSRC, "rays.cuh"),
     os.path.join(CSRC, "spec_kernel.cuh"),
     os.path.join(CSRC, "spec_tile_kernel.cuh"),
     os.path.join(CSRC, "reset.cuh"),

@@ -226,17 +226,45 @@ def _act_fields(act) -> list:
     return fields
 
 
-def post_hash(cols, instrs, acts=(), obs_dtype: int = 0) -> int:
+# ---- the LIDAR stage of the whole-step kernel's epilogue ------------------------------------------------------------
+#: the most targets one LIDAR of a whole-step kernel casts its rays at (``SPEC_LIDAR_MAX_TARGETS`` in
+#: csrc/spec_kernel.cuh: the epilogue unrolls every ray against every target).  A plan with a sensor that sees more
+#: stays on the captured graph, which casts them with ``cast_rays_batched_kernel``.
+MAX_LIDAR_TARGETS = 16
+
+
+def lidar_sensors(lidars, index_of, ray_targets):
+    """The LIDAR table of a whole-step kernel: ``(sensors, flip)`` for the ``lidars`` of ``ObservationPlan.compile``
+    (``[(row, first column, sensor, range_minus_distance)]``), or None if a sensor sees more than
+    ``MAX_LIDAR_TARGETS`` targets.  A sensor is ``(source entity, targets, angles, max_range, row, first column)``:
+    the targets in ``ray_targets`` order, the angles and the range as the fp32 values ``cast_rays_batched_kernel``
+    reads.  ``flip``: the readings are stored as ``max_range - distance`` (one setting per plan, as
+    ``backend.observe`` takes it)."""
+    sensors = []
+    for row, col, s, _ in lidars:
+        targets = tuple(int(t) for t in ray_targets(s.agent, s.entity_filter))
+        if len(targets) > MAX_LIDAR_TARGETS:
+            return None
+        angles = tuple(float(x) for x in np.asarray(s._angles[0].detach().cpu(), dtype=np.float32))
+        sensors.append((int(index_of(s.agent)), targets, angles, float(np.float32(s._max_range)), int(row), int(col)))
+    return tuple(sensors), bool(lidars[0][3]) if lidars else False
+
+
+def post_hash(cols, instrs, acts=(), obs_dtype: int = 0, lidar=None) -> int:
     """FNV-1a 64 of what a whole-step kernel does around the substeps: the observation plan's column table
     (int32 ``[rows, width, 4]`` or None), the step program's instructions ``[(op, dst, a, b, arg, imm)]`` with
     entity indices resolved, the action ingest of the policy agents (``prologue_acts``; empty: actions are ingested
-    by a launch of their own) and the type of the observation rows (``VMAS_DTYPE_*``; fp32 adds nothing to the
-    hash)."""
+    by a launch of their own), the type of the observation rows (``VMAS_DTYPE_*``; fp32 adds nothing to the
+    hash) and the LIDAR table (``lidar_sensors``; None or no sensor adds nothing)."""
     parts = [None if cols is None else [list(cols.shape), [int(x) for x in cols.reshape(-1)]],
              [[int(op), int(dst), int(a), int(b), int(arg), _f(imm)] for op, dst, a, b, arg, imm in instrs],
              [_act_fields(act) for act in acts]]
     if obs_dtype:
         parts.append(int(obs_dtype))
+    if lidar and lidar[0]:
+        sensors, flip = lidar
+        parts.append([int(flip), [[src, list(targets), [_f(a) for a in angles], _f(rng), row, col]
+                                  for src, targets, angles, rng, row, col in sensors]])
     blob = json.dumps(parts).encode()
     h = 0xCBF29CE484222325
     for byte in blob:
@@ -260,11 +288,12 @@ def fuse_value_columns(cols, buffer_sources, instrs):
     return cols
 
 
-def emit_post(cols, instrs, acts=(), obs_dtype: int = 0) -> Tuple[str, str, int]:
-    """C++ text of one epilogue (+ ingest prologue) struct (``spec_epilogue`` / ``spec_ingest`` in
+def emit_post(cols, instrs, acts=(), obs_dtype: int = 0, lidar=None) -> Tuple[str, str, int]:
+    """C++ text of one epilogue (+ ingest prologue) struct (``spec_epilogue`` / ``spec_ingest`` / ``spec_lidar`` in
     csrc/spec_kernel.cuh).  ``obs_dtype``: what the observation rows are stored as (``VMAS_DTYPE_F32`` = 0,
-    ``VMAS_DTYPE_F16`` = 1, ``VMAS_DTYPE_BF16`` = 2).  Returns (name, text, hash)."""
-    h = post_hash(cols, instrs, acts, obs_dtype)
+    ``VMAS_DTYPE_F16`` = 1, ``VMAS_DTYPE_BF16`` = 2).  ``lidar``: ``lidar_sensors`` of the plan's LIDAR terms (their
+    columns are SKIP in ``cols``).  Returns (name, text, hash)."""
+    h = post_hash(cols, instrs, acts, obs_dtype, lidar)
     name = f"Post_{h:016x}"
     rows, width = (0, 0) if cols is None else (int(cols.shape[0]), int(cols.shape[1]))
     lines = [f"struct {name} {{"]
@@ -298,6 +327,23 @@ def emit_post(cols, instrs, acts=(), obs_dtype: int = 0) -> Tuple[str, str, int]
             par_f = float(np.array([par], dtype=np.int32).view(np.float32)[0])
             lines.append(f"      {{{int(op)}, {int(src)}, {int(src2)}, {_f(par_f)}}},")
     lines.append("  };")
+    if lidar and lidar[0]:  # (members a plan without LIDAR terms does not have: its text stays as it was)
+        sensors, flip = lidar
+        n_rays = {len(angles) for _, _, angles, _, _, _ in sensors}
+        if len(n_rays) != 1:
+            raise ValueError("LIDARs of one observation plan must have the same number of rays")
+        R = n_rays.pop()
+        lines.append(f"  static constexpr int N_LIDAR = {len(sensors)}, LIDAR_RAYS = {R}, LIDAR_FLIP = {int(flip)};")
+        lines.append(f"  static constexpr LidarC lidar[{len(sensors)}] = {{")
+        for src, targets, angles, rng, row, col in sensors:
+            if len(targets) > MAX_LIDAR_TARGETS:
+                raise ValueError(f"a LIDAR of a whole-step kernel sees at most {MAX_LIDAR_TARGETS} targets")
+            lines.append(f"      {{{src}, {row}, {col}, {_f(rng)}, {len(targets)}, {{{', '.join(str(t) for t in targets)}}}}},")
+        lines.append("  };")
+        lines.append(f"  static constexpr float lidar_angle[{len(sensors) * R}] = {{")
+        for _, _, angles, _, _, _ in sensors:
+            lines.append("      " + ", ".join(_f(a) for a in angles) + ",")
+        lines.append("  };")
     lines.append("};")
     return name, "\n".join(lines), h
 

@@ -19,6 +19,7 @@
 #include "geometry.cuh"
 #include "ingest.cuh"
 #include "query.cuh"
+#include "rays.cuh"
 #include "vmas_b200.h"
 
 namespace vmas {
@@ -48,6 +49,15 @@ struct ProgC {
 struct ObsColC {
   int op, src, src2;  // as the observation gather's column codes: (field << 24) | element offset in the env's row
   float par;
+};
+// ... and its LIDAR stage (see spec_lidar): one sensor of the plan, its angles in P::lidar_angle
+constexpr int SPEC_LIDAR_MAX_TARGETS = 16;  // (codegen.MAX_LIDAR_TARGETS: a plan with more stays on the captured graph)
+static_assert(SPEC_LIDAR_MAX_TARGETS <= 32, "spec_lidar keeps a sensor's targets in reach as bits of one word");
+struct LidarC {
+  int src, row, col;  // the sensor's entity; its observation row and first column
+  float max_range;
+  int n_targets;
+  int target[SPEC_LIDAR_MAX_TARGETS];  // the entities its rays can hit, in backend.ray_targets order
 };
 struct EpiArgs {
   void* obs_out;  // [rows, B, width] of P::OBS_DTYPE (fp32, fp16 or bf16), or null
@@ -1075,6 +1085,79 @@ DEVI void spec_epilogue(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs
   }
 }
 
+// ---- the LIDAR stage of the epilogue --------------------------------------------------------------------------------
+// What cast_rays_batched_kernel does behind the observation launch of a plan with LIDAR terms, on the registers that
+// hold the env's state after the last substep: every ray of every sensor of P (P::N_LIDAR; a plan without LIDAR terms
+// has no such member and no code here), its reading stored into the sensor's columns of the observation rows.  Same
+// functions (rays.cuh), same targets in the same order, same reach test, same fp32(angle + rot) and sincosf, same
+// max_range - distance: the same bits.
+template <class P, class = void>
+struct EpiLidars {
+  static constexpr int N = 0;
+};
+template <class P>
+struct EpiLidars<P, std::void_t<decltype(P::N_LIDAR)>> {
+  static constexpr int N = P::N_LIDAR;
+};
+
+// target T of a sensor as the epilogue holds it: position in the registers, heading from epi_state, shape constants
+template <class W, int T>
+struct EpiRayTarget {
+  const EnvRegs<W::E>& r;
+  const SpecArgs& a;
+  long env;
+  DEVI int shape() const { return W::ent[T].shape; }
+  DEVI V2 pos() const { return mk(r.px[T], r.py[T]); }
+  DEVI float rot() const { return epi_state<W, VMAS_OBS_ROT, T>(r, a, env); }
+  DEVI float d0() const { return W::ent[T].d0; }
+  DEVI float d1() const { return W::ent[T].d1; }
+};
+
+// G lanes own the env: ray k of a sensor goes to lane k % G, which stores its column.  The rays of a sensor are a loop
+// (not unrolled: a sensor's target tests are emitted once, not once per ray, so that the kernel's code stays within
+// what the instruction caches hold); a ray's angle is picked from the compile-time table by its index.
+template <class W, class P, int G>
+DEVI void spec_lidar(const EnvRegs<W::E>& r, const SpecArgs& a, const EpiArgs& e, const long env, const bool odd) {
+  if constexpr (EpiLidars<P>::N > 0) {
+    constexpr int R = P::LIDAR_RAYS, F = P::OBS_WIDTH, DT = P::OBS_DTYPE;
+    static_for<P::N_LIDAR>([&](auto qi) {
+      using Q = decltype(qi);
+      constexpr LidarC L = P::lidar[Q::value];
+      const V2 o = mk(r.px[L.src], r.py[L.src]);
+      const float src_rot = epi_state<W, VMAS_OBS_ROT, L.src>(r, a, env);
+      // the exact early-out of the batched kernel's phase A: a bit per target within the sensor's reach
+      uint32_t reach = 0u;
+      static_for<L.n_targets>([&](auto ti) {
+        constexpr int t = P::lidar[Q::value].target[decltype(ti)::value];
+        if (ray_in_reach(o, mk(r.px[t], r.py[t]), W::ent[t].circ_r, P::lidar[Q::value].max_range))
+          reach |= 1u << decltype(ti)::value;
+      });
+      const size_t at = ((size_t)L.row * a.batch_dim + env) * F + L.col;
+#pragma unroll 1
+      for (int k = G > 1 && odd ? 1 : 0; k < R; k += G) {
+        float d = L.max_range;
+        if (reach) {
+          float angle = 0.f;
+          static_for<R>([&](auto ki) {
+            constexpr float value = P::lidar_angle[Q::value * R + decltype(ki)::value];
+            if (k == decltype(ki)::value) angle = value;
+          });
+          float ds, dc;
+          sincosf(angle + src_rot, &ds, &dc);
+          static_for<L.n_targets>([&](auto ti) {
+            constexpr int t = P::lidar[Q::value].target[decltype(ti)::value];
+            if ((reach >> decltype(ti)::value) & 1u)
+              d = tmin(d, ray_vs_shape(EpiRayTarget<W, t>{r, a, env}, o, dc, ds, P::lidar[Q::value].max_range));
+          });
+        }
+        const float v = P::LIDAR_FLIP ? L.max_range - d : d;
+        if constexpr (DT == VMAS_DTYPE_F32) static_cast<float*>(e.obs_out)[at + k] = v;
+        else static_cast<uint16_t*>(e.obs_out)[at + k] = obs16_bits<DT>(v);
+      }
+    });
+  }
+}
+
 // One env, all of `a.n_substeps` substeps, state in the calling thread's registers.  `P` (not void): the
 // step's epilogue runs behind the last substep (the whole-step kernel).
 template <class W, bool TRACK = false, class P = void>
@@ -1104,7 +1187,10 @@ DEVI void spec_env_step(const SpecArgs& a, const long env, const uint32_t (&mask
   }
   rows.store(a, env, r, afx, afy, atq);
   if constexpr (!std::is_void_v<P>) {
-    if (a.first_substep + a.n_substeps == W::cfg.substeps) spec_epilogue<W, P>(r, a, *epi, env);
+    if (a.first_substep + a.n_substeps == W::cfg.substeps) {
+      spec_epilogue<W, P>(r, a, *epi, env);
+      spec_lidar<W, P, 1>(r, a, *epi, env, false);
+    }
   }
   if constexpr (TRACK) {
     if (a.sig) a.sig[env] = (a.first_substep == 0 ? 0u : a.sig[env]) | sig;  // OR over the substeps of a step
@@ -1639,6 +1725,7 @@ __global__ void __launch_bounds__(W::BLOCK* G, (W::MIN_BLOCKS / G > 0 ? W::MIN_B
     spec_epilogue<W, P>(r, a, e, env, G, odd ? 1 : 0, from_lane0, [count](const float*) { return count; });
   else
     spec_epilogue<W, P>(r, a, e, env, G, odd ? 1 : 0, from_lane0);
+  spec_lidar<W, P, G>(r, a, e, env, odd);
   if constexpr (MW > 0) {
     // thread 0 (always live: it owns the block's first env) is the only thread that touches a.mask.  Once every
     // block has counted itself here, every block has arrived at every barrier and read every mask it waited for,

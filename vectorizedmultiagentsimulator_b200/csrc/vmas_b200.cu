@@ -25,6 +25,7 @@
 #include "generic_step.cuh"
 #include "query.cuh"
 #include "ingest.cuh"
+#include "rays.cuh"
 #include "generated/specializations.cuh"
 #include "vmas_b200.h"
 
@@ -487,90 +488,7 @@ __global__ void __launch_bounds__(32 * BROAD_SLICES) broad_phase_kernel(const St
 // ---------------------------------------------------------------------------------------------
 // LIDAR (ref core.py:1662-1786 and the three shape kernels 1281-1372, 1414-1490, 1544-1626)
 // ---------------------------------------------------------------------------------------------
-// torch.min / torch.max propagate NaN; fminf / fmaxf do not.
-DEVI float tmin(float x, float y) { return (x != x || y != y) ? NAN : fminf(x, y); }
-DEVI float tmax(float x, float y) { return (x != x || y != y) ? NAN : fmaxf(x, y); }
-
-struct RayArgs {
-  VmasWorldConfig cfg;
-  VmasPlanTables tb;
-  VmasState st;
-  const int32_t* targets;
-  const float* angles;
-  float* out;
-  int32_t src, n_targets, n_rays, add_rot_of;
-  float max_range;
-};
-
-// ref core.py:1414-1490
-DEVI float ray_vs_sphere(V2 o, float dc, float ds, V2 c, float radius, float max_range) {
-  const float half = max_range / 2.f;
-  V2 line_pos = mk(o.x + dc * half, o.y + ds * half);
-  V2 u = c - o;
-  if (!((u.x * dc + u.y * ds) > 0.f)) return max_range;  // behind the sensor
-  V2 closest = closest_point_carrier(line_pos, dc, ds, c);
-  float dn = norm2(c - closest);
-  if (!(dn < radius)) return max_range;  // the carrier passes the sphere by
-  float aa = radius * radius - dn * dn;
-  float m = sqrtf(aa > 0.f ? aa : 1e-8f);
-  return norm2(closest - o) - m;
-}
-
-DEVI float ray_vs_entity(const RayArgs& a, V2 o, float ang, float dc, float ds, int t, size_t env_base) {
-  const int shape = __ldg(a.tb.ent_i32 + t * 4);
-  const float* ef = a.tb.ent_f32 + (size_t)t * VMAS_EF_COLS;
-  const float2 tp = reinterpret_cast<const float2*>(a.st.pos)[env_base + t];
-  const V2 c = mk(tp.x, tp.y);
-  const float max_range = a.max_range;
-  if (shape == VMAS_SHAPE_SPHERE) return ray_vs_sphere(o, dc, ds, c, __ldg(ef + VMAS_EF_D0), max_range);
-  const float trot = a.st.rot[env_base + t];
-  if (shape == VMAS_SHAPE_BOX) {
-    const float L = __ldg(ef + VMAS_EF_D0), Wd = __ldg(ef + VMAS_EF_D1);
-    float sn, cs;
-    sincosf(-trot, &sn, &cs);
-    V2 ol = rot2(o - c, cs, sn);
-    V2 dl = rot2(mk(dc, ds), cs, sn);
-    float tx1 = (-L / 2.f - ol.x) / dl.x, tx2 = (L / 2.f - ol.x) / dl.x;
-    float t0 = tmin(tx1, tx2), t1 = tmax(tx1, tx2);
-    float ty1 = (-Wd / 2.f - ol.y) / dl.y, ty2 = (Wd / 2.f - ol.y) / dl.y;
-    float ty0 = tmin(ty1, ty2), tyM = tmax(ty1, ty2);
-    t0 = tmax(t0, ty0);
-    t1 = tmin(t1, tyM);
-    V2 hl = mk(t0 * dl.x + ol.x, t0 * dl.y + ol.y);
-    float sn2, cs2;
-    sincosf(trot, &sn2, &cs2);
-    V2 hw = rot2(hl, cs2, sn2) + c;
-    bool hit = (t1 >= t0) && (t0 > 0.f);
-    return hit ? norm2(o - hw) : max_range;
-  }
-  // line
-  {
-    const float L = __ldg(ef + VMAS_EF_D0);
-    float sn, cs;
-    sincosf(trot, &sn, &cs);
-    V2 r = mk(cs * L, sn * L);
-    V2 s = mk(dc, ds);
-    float rxs = cross2(r, s);
-    V2 qp = o - c;
-    float tt = cross2(qp, mk(s.x / rxs, s.y / rxs));
-    float uu = cross2(qp, mk(r.x / rxs, r.y / rxs));
-    float d = norm2(uu * s.x, uu * s.y);
-    bool miss = (rxs == 0.f) || (tt > 0.5f) || (tt < -0.5f) || (uu < 0.f);
-    return miss ? max_range : d;
-  }
-}
-
-// Exact early-out shared by both ray kernels: a target whose circumscribed circle lies beyond the
-// sensor's range cannot shorten a ray (any hit distance is >= |c - o| - circ_r > max_range, and the
-// result is min(max_range, ...)), so its shape test — and, when no target is in reach, the ray's
-// sin/cos — is skipped.  The margin dwarfs fp32 rounding of the skipped arithmetic.
-DEVI bool ray_target_in_reach(const RayArgs& a, V2 o, int t, size_t env_base) {
-  const float2 tp = reinterpret_cast<const float2*>(a.st.pos)[env_base + t];
-  const float reach = (a.max_range + __ldg(a.tb.ent_f32 + (size_t)t * VMAS_EF_COLS + VMAS_EF_CIRC_R)) * 1.001f + 1e-3f;
-  const float dx = tp.x - o.x, dy = tp.y - o.y;
-  return !(dx * dx + dy * dy > reach * reach);  // NaN positions stay "in reach"
-}
-
+// (one ray against one target: rays.cuh)
 template <class TargetAt>
 DEVI float cast_one_ray(const RayArgs& a, float ang, int n_targets, TargetAt target_at, size_t env_base) {
   const float2 op = reinterpret_cast<const float2*>(a.st.pos)[env_base + a.src];

@@ -93,7 +93,7 @@ _keepalive = []  # loaded objects must outlive the registry entries that point i
 def _source_stamp() -> str:
     """Hash of the headers the object is compiled from: a header edit invalidates the cache."""
     h = hashlib.sha1()
-    for name in ("geometry.cuh", "query.cuh", "ingest.cuh", "spec_kernel.cuh", "spec_tile_kernel.cuh"):
+    for name in ("geometry.cuh", "query.cuh", "ingest.cuh", "rays.cuh", "spec_kernel.cuh", "spec_tile_kernel.cuh"):
         h.update(open(os.path.join(_native.CSRC, name), "rb").read())
     h.update(open(os.path.join(_native.INCLUDE, "vmas_b200.h"), "rb").read())
     return h.hexdigest()[:12]
@@ -196,16 +196,17 @@ class StepKernelJob(Job):
     """The whole-step kernel of one (world, observation columns, step program): ``index`` is the handle for
     ``VmasEnvStep.fused_kernel`` once ``done`` is set."""
 
-    def __init__(self, desc: P.WorldDescription, cols, instrs, acts=(), out_dir: Optional[str] = None, obs_dtype: int = 0):
+    def __init__(self, desc: P.WorldDescription, cols, instrs, acts=(), out_dir: Optional[str] = None, obs_dtype: int = 0,
+                 lidar=None):
         super().__init__(desc, out_dir)
-        self.cols, self.instrs, self.acts, self.obs_dtype = cols, instrs, tuple(acts), int(obs_dtype)
-        self.post_hash = codegen.post_hash(cols, instrs, self.acts, self.obs_dtype)
+        self.cols, self.instrs, self.acts, self.obs_dtype, self.lidar = cols, instrs, tuple(acts), int(obs_dtype), lidar
+        self.post_hash = codegen.post_hash(cols, instrs, self.acts, self.obs_dtype, lidar)
         self.key = (self.hash ^ ((self.post_hash << 1) | (self.post_hash >> 63))) & 0xFFFFFFFFFFFFFFFF
 
     def _compile_and_register(self) -> int:
         desc = self.desc
         name, text, h = codegen.emit_world(desc, "whole-step kernel")
-        post_name, post_text, _ = codegen.emit_post(self.cols, self.instrs, self.acts, self.obs_dtype)
+        post_name, post_text, _ = codegen.emit_post(self.cols, self.instrs, self.acts, self.obs_dtype, self.lidar)
         stem = f"step_{self.key:016x}_{_native.ARITH}_{_source_stamp()}"
         source = _STEP_TEMPLATE.format(world=text, post=post_text, name=name, post_name=post_name)
         obj = C.CDLL(_shared_object(stem, source, self.out_dir))
@@ -226,15 +227,16 @@ _step_jobs: Dict[int, StepKernelJob] = {}
 
 
 def request_step_kernel(desc: P.WorldDescription, cols, instrs, acts=(), block: bool = False,
-                        obs_dtype: int = 0) -> Optional[StepKernelJob]:
+                        obs_dtype: int = 0, lidar=None) -> Optional[StepKernelJob]:
     """Starts (or finds) the compilation of the whole-step kernel; None if the world cannot be specialised or
     has per-env physical parameters (those step on the captured graph of the specialised substep kernel).
     ``acts``: ``codegen.prologue_acts`` of the policy agents if the kernel is to ingest their actions itself.
     ``prebuild_step_kernels`` compiles the continuous variants only.  ``obs_dtype``: the type the kernel stores its observation
-    rows as (``VMAS_DTYPE_*``; part of the key)."""
+    rows as (``VMAS_DTYPE_*``; part of the key).  ``lidar``: ``codegen.lidar_sensors`` of the plan's LIDAR terms, cast
+    in the epilogue (part of the key)."""
     if not available() or not codegen.specializable(desc):
         return None
-    job = StepKernelJob(desc, cols, instrs, acts, obs_dtype=obs_dtype)
+    job = StepKernelJob(desc, cols, instrs, acts, obs_dtype=obs_dtype, lidar=lidar)
     with _lock:
         have = _step_jobs.get(job.key)
         if have is None:

@@ -918,7 +918,9 @@ class Environment(TorchVectorizedObject):
         step consists of nothing but this library's ``World.step`` followed by one step program / observation
         launch — the graph then holds no torch kernel, and ``vmas_b200_env_step`` can issue those launches
         itself (direct mode), or one whole-step kernel.  ``limit``: ``(StepProgram, struct)`` of the environment's
-        step limit if its launch follows (``_limit_program``), else None.  None otherwise."""
+        step limit if its launch follows (``_limit_program``), else None.  The observation launch may be followed by the
+        plan's LIDAR launch (``backend.observe`` issues it from the same call, for exactly the plan's LIDAR terms).
+        None otherwise."""
         kinds = None if trace is None else [t[0] for t in trace]
         if not _DIRECT_STEP or kinds not in (["step", "post"], ["step", "post", "post"]):
             return None
@@ -931,8 +933,10 @@ class Environment(TorchVectorizedObject):
                 return None  # (a second program of the scenario's)
             limit = (lprog, lc)
         values = plan is not None and bool(plan.buffer_sources)  # columns fed by the program: program, then gather
-        if n_post != (2 if values and prog is not None else 1) or n_step + n_post + n_limit != self._graph_launches:
-            return None  # (LIDAR columns ride in a launch of their own; anything else the backend launched)
+        lidars = plan is not None and bool(plan.compile(self.world)[1])
+        n_want = (2 if values and prog is not None else 1) + (1 if lidars else 0)
+        if n_post != n_want or n_step + n_post + n_limit != self._graph_launches:
+            return None  # (anything else the backend launched)
         if values and any(not hasattr(src, "_slot") or src not in prog.outputs for src in plan.buffer_sources):
             return None  # (value columns that are not outputs of this program)
         backend = self.world._get_backend()
@@ -945,7 +949,9 @@ class Environment(TorchVectorizedObject):
         cols = None
         if plan is not None:
             dev = plan.device_cache.get(id(backend))
-            cols = dev["cols"] if dev is not None and dev["any_state"] else None
+            # (a plan with LIDAR terms keeps its column table even without state columns: the whole-step kernel writes
+            # the readings into its rows)
+            cols = dev["cols"] if dev is not None and (dev["any_state"] or lidars) else None
         return mode, c, prog, plan, cols, out, limit
 
     def _splice_limit(self, c, prog, instrs, limit):
@@ -1012,7 +1018,9 @@ class Environment(TorchVectorizedObject):
                 spliced = self._splice_limit(direct[1], direct[2], direct[2].instructions(backend.index_of), direct[6])
             if spliced is None:
                 direct = None  # (too large a program, or no counter: the step stays on the graph)
-        job = None
+        job, lidar_terms = None, []
+        if direct is not None and direct[3] is not None:
+            lidar_terms = direct[3].compile(self.world)[1]
         if direct is None:
             plan = N.EnvStepPlan(
                 backend.lib, backend._dev_tables, self.world.slab, arr, len(live), self.clamp_action,
@@ -1065,14 +1073,20 @@ class Environment(TorchVectorizedObject):
                     acts = codegen.prologue_acts(arr, N.ACT_CONTINUOUS if self.continuous_actions else int(arr[0].action_kind))
                     if acts:
                         plan.c.ingest_in_kernel = 1
-                job = jit.request_step_kernel(backend.tables.desc, cols_np, instrs, acts, obs_dtype=obs_dtype)
+                # the plan's LIDARs are cast in the kernel's epilogue (None: a sensor sees more targets than it takes)
+                lidar = codegen.lidar_sensors(lidar_terms, backend.index_of, backend.ray_targets) if lidar_terms else None
+                if lidar is not None or not lidar_terms:
+                    job = jit.request_step_kernel(backend.tables.desc, cols_np, instrs, acts, obs_dtype=obs_dtype,
+                                                  lidar=lidar)
                 if job is not None:
                     job.done.wait(timeout=_WHOLE_STEP_KERNEL_WAIT_S)
-        if direct is not None and direct[3] is not None and direct[3].buffer_sources and not (
+            plan.measurements = self._lidar_measurements(lidar_terms, obs_to, oplan)
+        if direct is not None and direct[3] is not None and (direct[3].buffer_sources or lidar_terms) and not (
             job is not None and job.done.is_set() and job.index > 0
         ):
-            # value columns need the program and the gather in ONE thread: without the whole-step kernel the
-            # step stays a captured graph (program launch, then gather launch)
+            # value columns need the program and the gather in ONE thread, and the direct launches have no LIDAR
+            # launch: without the whole-step kernel the step stays a captured graph (program launch, then gather
+            # launch, then the LIDAR launch)
             return self._build_one_call_step(graph, ingest_built_mask, None)
         plan.direct = direct is not None
         plan.job = job
@@ -1143,6 +1157,19 @@ class Environment(TorchVectorizedObject):
         c2.n_instr = len(instrs) + len(extra)
         return c2, instrs + extra, rest, obs_to, mirrors
 
+    def _lidar_measurements(self, lidar_terms, obs_to, oplan):
+        """What a one-call step makes of ``Lidar._last_measurement``: None when the readings land where the graph
+        path put them (the static observation block), else ``(block, first element, shape, [(sensor, row, column,
+        rays)])`` of the readings in the step's fresh result block.  In an fp32 block an unflipped sensor's entry is
+        a view of its readings, as ``backend.observe`` leaves it; a flipped sensor gets None, as there.  A 16-bit
+        block holds no fp32 readings: every sensor gets None."""
+        if not lidar_terms or obs_to is None:
+            return None
+        block, offset = obs_to
+        fp32 = not self._graph_out_block_kinds[block]
+        sensors = [(s, r, c, int(s._angles.shape[1]) if fp32 and not flipped else 0) for r, c, s, flipped in lidar_terms]
+        return block, offset // 4 if fp32 else None, (oplan.n_rows, self.num_envs, oplan.width), sensors
+
     def _adopt_whole_step_kernel(self, plan):
         job = plan.job
         if job is None or not job.done.is_set():
@@ -1172,6 +1199,12 @@ class Environment(TorchVectorizedObject):
         for j, c in enumerate(copies):
             blocks[j] = c.data_ptr()
         launched = plan.run()  # (the kernels the call issued itself; a graph's nodes come on top)
+        measured = getattr(plan, "measurements", None)
+        if measured is not None:
+            block, first, shape, sensors = measured
+            rows = None if first is None else copies[block][first : first + math.prod(shape)].view(shape)
+            for sensor, r, c, n in sensors:
+                sensor._last_measurement = rows[r, :, c : c + n] if n else None
         for action, u in plan.bind:  # (a reset replaces agent.action.u; the call writes the static buffers)
             if action._u is not u:
                 action.u = u
